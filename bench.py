@@ -1,8 +1,8 @@
 #!/usr/bin/env python
-"""bench.py -- the driver's measurement contract for the ReChorus training hot path on B200.
+"""bench.py -- measures the ReChorus training hot path on H100 GPUs.
 
     python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--workload c1|c2|c3|c4|c5]
-                    [--headline_only] [--no_cpu_baseline]
+                    [--headline_only] [--no_cpu_baseline] [--dump-outputs DIR]
 
 A "step" is one pass of the hot path over one batch of synthetic input: forward (gather + interaction), BPR loss,
 backward and the optimizer update -- the body of helpers/BaseRunner.py:193-206.  metric = training samples/s counted as
@@ -13,7 +13,7 @@ Workloads = BASELINE.json configs, in order:
   c2  BPRMF d=64, 1 M users x 1 M items, K=99, B=4096                       <- the headline (metric is quoted on it)
   c3  NeuMF d=64, MLP [64,32,16], K=4, B=4096, 1 M x 1 M
   c4  SASRec L=50 d=64, 2 blocks, 4 heads, K=99, B=4096, 1 M items
-  c5  BPRMF d=128, 100 M items (1 M users) row-range sharded over the ranks, K=255, B=4096 per GPU
+  c5  BPRMF d=128, 25 M items (1 M users) row-range sharded over the ranks, K=255, B=4096 per GPU
 Default: N=1 -> the c2 line, with compact lines of c1/c3/c4/c5 (c5 on one GPU, the anchor of its scaling curve) under
 "workloads".  N>1 -> the sharded c5 over N ranks (configs 1-4 do not shard: replicas of them measure nothing); rank 0
 then repeats c5 alone on its GPU ("n1_same_code") so that every N>1 line carries its own 1-GPU anchor.
@@ -21,7 +21,12 @@ then repeats c5 alone on its GPU ("n1_same_code") so that every N>1 line carries
 Prints ONE JSON line (rank 0).  `value`: inputs already resident in HBM.  `e2e`: the same step through the public plugin
 call with the batch coming from pinned host memory every step and the loss read back every step.  `roofline`: dominant
 kernel, algorithmic bytes / CUDA-event time / measured peak.  `cpu_baseline`: the reference's own classes through its
-own BaseRunner.fit on this box's host cores (kind "reference", from baseline/_ref), else the oracle port.
+own BaseRunner.fit on the host cores (kind "reference", from the unmodified copy build() stages in oracle/_ref), else the
+oracle port.
+
+--dump-outputs DIR: after the timed steps, write what the timed path computed in its last step as DIR/<name>.npy
+(float32): the loss (c1: the timed epoch's mean loss), and the model's parameters (c5: rank 0's row shards) -- a fixed,
+seeded sample of rows for the embedding tables, which are too large to store whole.  Inputs and initial weights are seeded, so two builds can be compared output for output.
 """
 from __future__ import annotations
 
@@ -51,8 +56,9 @@ WORKLOADS = {
                desc="NeuMF (GMF + MLP [64,32,16]) emb_dim=64, 1M users x 1M items, num_neg=4, batch=4096"),
     "c4": dict(model="SASRec", n_users=1_000_000, n_items=1_000_000, d=64, B=4096, K=99, L=50, blocks=2, heads=4,
                desc="SASRec history_max=50 emb_dim=64, 2 blocks, 4 heads, 1M items, num_neg=99, batch=4096"),
-    "c5": dict(model="BPRMF", n_users=1_000_000, n_items=100_000_000, d=128, B=4096, K=255,
-               desc="BPRMF emb_dim=128, 100M synthetic items (1M users) row-range sharded, num_neg=255, batch=4096 per GPU"),
+    # 25 M x 128 floats = 12.8 GB of table + 25.6 GB of Adam state: the whole problem fits one 80 GB H100
+    "c5": dict(model="BPRMF", n_users=1_000_000, n_items=25_000_000, d=128, B=4096, K=255,
+               desc="BPRMF emb_dim=128, 25M synthetic items (1M users) row-range sharded, num_neg=255, batch=4096 per GPU"),
 }
 METRIC = "training samples/sec (user x (1+neg))"
 UNIT = "user*item/s"
@@ -65,12 +71,12 @@ def measured_peaks():
     if os.path.exists(path):
         with open(path) as f:
             p = json.load(f)
-        return float(p["hbm_gbs"]), float(p.get("bf16_tflops", 1729.8)), "measured (MEASURED_PEAKS.json)"
-    return 6650.0, 1730.0, "fallback (B200_PROFILING.md: 6.65 TB/s copy, 1.73 PFLOP/s bf16)"
+        return float(p["hbm_gbs"]), float(p.get("bf16_tflops", 989.0)), "measured (MEASURED_PEAKS.json)"
+    return 3350.0, 989.0, "fallback (H100 SXM data sheet: 3.35 TB/s HBM3, 989 TFLOP/s dense bf16; not measured)"
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons sampled DURING the timed region (B200_PROFILING.md recipe)."""
+    """nvidia-smi clocks / throttle reasons sampled DURING the timed region."""
     Q = ("clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.hw_slowdown,"
          "clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,"
          "clocks_event_reasons.sw_power_cap")
@@ -102,11 +108,13 @@ class ClockSampler:
     def stop(self) -> dict:
         if self.proc is None:
             return {"sm_mhz": None, "sm_max_mhz": None, "reasons": ["nvidia-smi unavailable"]}
-        self.proc.terminate()          # exact PID we started
-        try:
-            self.proc.wait(timeout=5)
-        except subprocess.TimeoutExpired:
-            self.proc.kill()
+        if self.proc.poll() is None:
+            self.proc.terminate()          # exact PID we started
+            try:
+                self.proc.wait(timeout=5)
+            except subprocess.TimeoutExpired:
+                self.proc.kill()
+                self.proc.wait()
         sm, mx, reasons = [], [], set()
         names = ["hw_slowdown", "hw_thermal_slowdown", "sw_thermal_slowdown", "sw_power_cap"]
         for ts, ln in self.lines:
@@ -202,6 +210,24 @@ class Dist:
         return ms
 
 
+DUMP_ROWS = 16384      # rows per embedding table written by --dump-outputs
+
+
+def dump_outputs(path, loss, named_params):
+    """--dump-outputs: the last timed step's loss and the model's parameters as float32 .npy files; a table with more than
+    DUMP_ROWS rows is written as the same seeded sample of DUMP_ROWS rows (sorted ids) on every run"""
+    os.makedirs(path, exist_ok=True)
+    arrays = {"loss": torch.as_tensor(loss).detach().reshape(())}
+    for name, t in named_params:
+        t = t.detach()
+        if t.dim() == 2 and t.shape[0] > DUMP_ROWS:
+            idx = torch.randperm(t.shape[0], generator=torch.Generator().manual_seed(0))[:DUMP_ROWS].sort().values
+            t = t.index_select(0, idx.to(t.device))
+        arrays[name] = t
+    for name, t in arrays.items():
+        np.save(os.path.join(path, name + ".npy"), t.float().cpu().numpy())
+
+
 def timed_loop(dist, fn, steps, warmup, k0=0):
     """W untimed + exactly K timed steps bracketed by barrier + synchronize; CUDA events; max over ranks"""
     for k in range(warmup):
@@ -279,6 +305,8 @@ def run_c2(args, rank, world, local_rank, sampler):
     host_ms_step = (time.time() - w0) * 1e3 / args.steps       # host time to enqueue a step (no sync inside the loop)
     dist.barrier()
     sampler.window(w0, time.time())
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, loss, model.named_parameters())
     launches = lib.b2r_launch_count() - launches0
     ms_step = dist.max_ms(t0.elapsed_time(t1)) / args.steps
     value = world * B * C / (ms_step * 1e-3)
@@ -561,7 +589,7 @@ def run_model_steps(wname, args, rank, world, local_rank, sampler, steps_cap):
     host = make_batches(w, seed=2000 + rank, pool=4)
     feeds = [to_feed(f, device, B) for f in host]
     pinned = [to_feed(f, device, B, pin=True) for f in host]
-    steps, warmup = max(3, min(args.steps, steps_cap)), max(3, min(args.warmup, 5))
+    steps, warmup = max(1, min(args.steps, steps_cap)), max(3, min(args.warmup, 5))
 
     def step(k):
         f = feeds[k % len(feeds)]
@@ -588,6 +616,8 @@ def run_model_steps(wname, args, rank, world, local_rank, sampler, steps_cap):
         import traceback
         traceback.print_exc(file=sys.stderr)
         gstep, ms = None, ms_eager
+    if args.dump_outputs and rank == 0 and wname == args.workload:
+        dump_outputs(args.dump_outputs, loss, model.named_parameters())
 
     def step_e2e(k):
         if gstep is None:                              # eager fallback: H2D of the pinned batch, then the same step
@@ -671,6 +701,8 @@ def run_c1(args, rank, world, local_rank, sampler):
         t_dev = time.time() - t0
         sampler.window(t0, time.time())
         n_steps = (len(data) + B - 1) // B
+    if args.dump_outputs and rank == 0 and args.workload == "c1":      # the epoch timed last: its mean loss, the tables
+        dump_outputs(args.dump_outputs, loss if loss_dev is None else loss_dev, model.named_parameters())
     ops.check_ids(device)
     rows = len(data)
     hbm, _, src = measured_peaks()
@@ -712,10 +744,12 @@ def run_c5(args, rank, world, local_rank, sampler, steps_cap, group=None, solo=F
             for _ in range(4)]
     pool = [(u.to(device), i.to(device)) for u, i in host]
     pinned = [(u.pin_memory(), i.pin_memory()) for u, i in host]
-    steps, warmup = max(3, min(args.steps, steps_cap)), max(3, min(args.warmup, 5))
+    steps, warmup = max(1, min(args.steps, steps_cap)), max(3, min(args.warmup, 5))
     launches0 = lib.b2r_launch_count()
     ms, loss, win = timed_loop(dist, lambda k: m.train_step(*pool[k % 4]), steps, warmup)
     launches = lib.b2r_launch_count() - launches0
+    if args.dump_outputs and rank == 0 and args.workload == "c5" and not solo:   # rank 0's row shards of both tables
+        dump_outputs(args.dump_outputs, loss, [("u_embeddings_shard0", m.U), ("i_embeddings_shard0", m.I)])
     sampler.window(*win)
 
     def step_e2e(k):
@@ -734,9 +768,9 @@ def run_c5(args, rank, world, local_rank, sampler, steps_cap, group=None, solo=F
            "n_gpus": eff_world,
            "config": {"workload": "c5: " + w["desc"], "optimizer": "Adam lr=1e-3 (row-sparse/lazy, fused)",
                       "parallelism": f"row-range shards x{eff_world}, score routing" if eff_world > 1 else
-                                     "single GPU holds the whole table (51.2 GB) + Adam state (102 GB), no collectives",
+                                     "single GPU holds the whole table (12.8 GB) + Adam state (25.6 GB), no collectives",
                       "exchange": m.exchange_description() if hasattr(m, "exchange_description") else "NCCL all-to-all",
-                      "l2_policy": "inputs larger than L2 (6.4+ GB of table per GPU), fresh ids every step"},
+                      "l2_policy": f"inputs larger than L2 ({12.8 / eff_world:.1f} GB of item table per GPU), fresh ids every step"},
            "e2e": {"value": round(eff_world * B * C / (ms_e2e * 1e-3), 1), "unit": UNIT, "ms_per_step": round(ms_e2e, 5),
                    "h2d_bytes_per_step": 8 * B + 8 * B * C, "d2h_bytes_per_step": 4},
            "gpu_launches": int(launches), "final_loss": round(float(loss), 6),
@@ -762,7 +796,7 @@ CPU_SAMPLE = {   # bounded samples: (steps, n_items override, note)
     "c4": dict(steps=2, note="full-size steps (B=4096, C=100, L=50)"),
     "c5": dict(steps=3, n_items=2_000_000, n_users=1_000_000,
                note="steps of B=4096, C=256, d=128 with the item table cut to 2 M rows: the reference's dense gradient + "
-                    "dense Adam over 100 M x 128 would need 205 GB of host memory and minutes per step (its cost grows with "
+                    "dense Adam over 25 M x 128 would need 51 GB of host memory and seconds per step (its cost grows with "
                     "the table; the cut favours the CPU)"),
 }
 
@@ -805,7 +839,7 @@ def cpu_leg(wname, steps_override=None):
     r = ref_arm.port_steps(w["model"], params, batches)
     return {"value": round(B * C * r["steps"] / r["loop_s"], 1), "unit": UNIT, "cores": cores, "os_cpu_count": os.cpu_count(),
             "kind": "port", "ms_per_step": round(r["loop_s"] * 1e3 / r["steps"], 2),
-            "sample": f"{r['steps']} " + s["note"] + "; oracle port of BaseRunner.py:184-207 (the reference tree is not on this box)"}
+            "sample": f"{r['steps']} " + s["note"] + "; oracle port of BaseRunner.py:184-207 (no staged reference in oracle/_ref)"}
 
 
 def run_reference_arm(args, rank):
@@ -835,6 +869,8 @@ def main():
     ap.add_argument("--workload", type=str, default="", choices=[""] + sorted(WORKLOADS))
     ap.add_argument("--no_cpu_baseline", action="store_true", help="skip the CPU legs (dev runs)")
     ap.add_argument("--headline_only", action="store_true", help="N=1: only the headline workload, no per-config block")
+    ap.add_argument("--dump-outputs", dest="dump_outputs", metavar="DIR", default="",
+                    help="after the timed steps, write the last step's loss and parameters as DIR/<name>.npy")
     args = ap.parse_args()
     args.warmup = max(args.warmup, 3) if args.impl == "ours" else args.warmup
 
@@ -858,6 +894,16 @@ def main():
         torch.distributed.init_process_group("nccl", device_id=device)
     sampler = ClockSampler(local_rank)
     sampler.start()
+    try:
+        run_workloads(args, rank, world, local_rank, explicit, device, sampler)
+    finally:
+        sampler.stop()                   # never leave the nvidia-smi child running (stop() is idempotent)
+    if world > 1:
+        torch.distributed.barrier()
+        torch.distributed.destroy_process_group()
+
+
+def run_workloads(args, rank, world, local_rank, explicit, device, sampler):
     time.sleep(0.3)                      # let nvidia-smi come up before the timed regions
 
     wl = args.workload
@@ -884,7 +930,7 @@ def main():
                 try:
                     a1 = run_c5(args, rank, world, local_rank, sampler, steps_cap=min(args.steps, 30), solo=True)
                     out["n1_same_code"] = {k: a1[k] for k in ("value", "ms_per_step", "steps", "mem_GB", "roofline")}
-                except Exception as e:                                   # e.g. a GPU without 155 GB free
+                except Exception as e:                                   # e.g. a GPU without 40 GB free
                     out["n1_same_code"] = {"unavailable": repr(e)[:200]}
             torch.distributed.barrier()
     if rank == 0 and world == 1 and wl == "c2" and not explicit and not args.headline_only:
@@ -924,9 +970,6 @@ def main():
                     except Exception as e:
                         r["cpu_baseline"] = {"error": repr(e)[:300]}
         print(json.dumps(out), flush=True)
-    if world > 1:
-        torch.distributed.barrier()
-        torch.distributed.destroy_process_group()
 
 
 if __name__ == "__main__":

@@ -1,4 +1,4 @@
-/* b200rec.h -- C ABI of libb200rec.so: the ReChorus training hot path as sm_100a CUDA kernels.
+/* b200rec.h -- C ABI of libb200rec.so: the ReChorus training hot path as sm_90a (H100) CUDA kernels.
  *
  * The reference (THUwangcy/ReChorus) has no FFI: its hot path is Python calling ATen.  Each entry point below
  * names the reference code it replaces (paths relative to the reference's src/).  The Python plugin layer
@@ -41,7 +41,7 @@ typedef void* b2r_stream_t;      /* cudaStream_t */
 
 B2R_API int         b2r_version(void);
 B2R_API const char* b2r_last_error(void);
-/* sm count / compute capability of the current device (148 / 10.0 on B200) */
+/* sm count / compute capability of the current device (132 / 9.0 on an H100 SXM) */
 B2R_API int         b2r_device_info(int* sm_count, int* cc_major, int* cc_minor);
 
 /* Measurement hooks for bench.py (no effect on results):
@@ -246,8 +246,8 @@ B2R_API int b2r_dense_optim(float* W, const float* grad, float* m, float* v, int
  * ---------------------------------------------------------------------------------------------- */
 B2R_API int b2r_linear_fwd(const float* X, int ldx, const float* W, const float* bias, float* Y, int ldy,
                    int64_t M, int N, int K, int relu, b2r_stream_t stream);
-/* Same forward on the tensor cores: tcgen05.mma kind::tf32 with the accumulator in TMEM and a 4-product hi/lo operand
- * split (error ~2^-21 relative, i.e. fp32 class).  K % 32 == 0 (<= 128), N % 16 == 0 (<= 256), contiguous W.  Returns
+/* Same forward on the tensor cores: wgmma.mma_async with TF32 operands, the accumulator in registers and a 3-product
+ * hi/lo operand split (error ~2^-21 relative, i.e. fp32 class).  K % 32 == 0 (<= 128), N % 16 == 0 (<= 256), contiguous W.  Returns
  * B2R_E_UNSUPPORTED outside that class. */
 B2R_API int b2r_linear_fwd_tc(const float* X, int ldx, const float* W, const float* bias, float* Y, int ldy,
                       int64_t M, int N, int K, int relu, b2r_stream_t stream);
@@ -262,7 +262,7 @@ B2R_API int b2r_linear_bwd_weight(const float* dY, int lddy, const float* relu_o
                           float* dW, float* dbias, int64_t M, int N, int K, void* ws, size_t ws_bytes,
                           b2r_stream_t stream);
 
-/* The same weight gradient on the tcgen05 tensor cores (kind::tf32 with a hi/lo operand split, accumulator in TMEM; the
+/* The same weight gradient on the tensor cores (wgmma TF32 with a hi/lo operand split, accumulator in registers; the
  * batch-row index is the MMA's reduction dimension, activations are transposed on their way into shared memory).
  * Shape class: N % 4 == 0, N <= 128, K % 16 == 0, K <= 240; returns B2R_E_UNSUPPORTED otherwise. */
 B2R_API size_t b2r_linear_bwd_weight_tc_workspace_bytes(int64_t M, int N, int K);

@@ -1,8 +1,8 @@
-"""Build libb200rec.so in-tree with nvcc for sm_100a (cross-compiles without a GPU).
+"""Build libb200rec.so in-tree with nvcc for sm_90a (H100; cross-compiles without a GPU).
 
     python -m rechorus_b200.build [--force] [--verbose]
 
-The .so is git-ignored but travels to the GPU box with the gpurun snapshot.  Objects go to build/.
+The .so is git-ignored and rebuilt from source by every checkout.  Objects go to build/.
 """
 from __future__ import annotations
 
@@ -19,7 +19,7 @@ OBJ_DIR = os.path.join(ROOT, "build", "obj")
 LIB_PATH = os.path.join(PKG, "libb200rec.so")
 
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
-ARCH = ["-gencode", "arch=compute_100a,code=sm_100a"]
+ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]
 CFLAGS = ["-O3", "-std=c++17", "-lineinfo", "-Xcompiler", "-fPIC", "-Xcompiler", "-fvisibility=hidden",
           "--expt-relaxed-constexpr", "-Xptxas", "-v"]
 

@@ -1,4 +1,4 @@
-// common.cuh -- shared device/host helpers for libb200rec.so (sm_100a only).
+// common.cuh -- shared device/host helpers for libb200rec.so (sm_90a only).
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -56,7 +56,7 @@ static inline size_t align_up(size_t x, size_t a) { return (x + a - 1) / a * a; 
 // ---- device helpers ---------------------------------------------------------------------------------
 
 // streaming 128-bit load of a table row chunk: read-only path, do not allocate in L1 (each row chunk is
-// used once per CTA; reuse across CTAs is served by the 126 MB L2)
+// used once per CTA; reuse across CTAs is served by the 50 MB L2)
 __device__ __forceinline__ float4 ld_row4(const float* p) {
     float4 r;
     asm volatile("ld.global.nc.L1::no_allocate.v4.f32 {%0, %1, %2, %3}, [%4];"

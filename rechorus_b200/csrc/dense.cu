@@ -3,8 +3,8 @@
 // the three layouts a Linear layer needs (forward, dX, dW with a deterministic split over the batch
 // dimension), residual + LayerNorm forward/backward, and fixed-order partial reductions.
 //
-// fp32 FMA on the CUDA cores keeps the 1e-5 parity bar of the north star; the tcgen05 (3xTF32) version of
-// the SASRec GEMMs is the tensor-pipe follow-up named in DESIGN.md.
+// fp32 FMA on the CUDA cores keeps the 1e-5 parity bar of the north star; linear_tc.cu and linear_dw_tc.cu are the
+// tensor-core (3xTF32 / 4xTF32 wgmma) versions for long batches.
 #include "common.cuh"
 
 namespace b2r {

@@ -1,37 +1,25 @@
-// linear_dw_tc.cu -- the weight gradient of nn.Linear on the 5th-generation tensor cores (tcgen05.mma kind::tf32,
-// accumulator in TMEM): dW[n, k] = sum_m dY[m, n] * X[m, k], dbias[n] = sum_m dY[m, n], the autograd of
+// linear_dw_tc.cu -- the weight gradient of nn.Linear on the Hopper tensor cores (wgmma.mma_async, TF32 operands, fp32
+// accumulator in registers): dW[n, k] = sum_m dY[m, n] * X[m, k], dbias[n] = sum_m dY[m, n], the autograd of
 // utils/layers.py:26-28,106-107 and NeuMF.py:70 behind loss.backward() (helpers/BaseRunner.py:205).
 //
-// Why this one first: in a SASRec step (config 4) the weight gradients are contractions over M = B*L = 204,800 rows with
-// a 64 x 64 result -- on the CUDA cores they were 27 % of the step (k_gemm<1,1>, 241 us each), more than the attention.
-// As a tensor-core problem they are an outer-product accumulation: D[128 x (K+16)] += A[128 x 32] * B[(K+16) x 32]^T per
-// 32-row slab, where A's rows are the N output features (rows N..127 stay zero), B's rows the K input features plus one
-// row of ones (its column of D is dbias), and the MMA's reduction dimension is the batch-row index m.  The operands are
-// therefore the TRANSPOSES of the row-major activations; they are transposed on the way into shared memory (each lane owns
-// one batch row of a slab and writes its elements down a column of the K-major SWIZZLE_128B tile: 32 lanes, 32 distinct
-// banks), split x = hi + lo (both TF32-exact) as in linear_tc.cu, and four products accumulate in one TMEM tile across the
-// CTA's whole row range.  One tcgen05.ld epilogue per CTA writes a partial [N x (K+16)] tile; a second kernel adds the
-// CTAs' partials in CTA order (fixed order -> deterministic).
+// In a SASRec step the weight gradients are contractions over M = B*L rows (hundreds of thousands) with a small result
+// (64 x 64), which on the CUDA cores cost more than the attention.  As a tensor-core problem they are an outer-product
+// accumulation: D[64 x NB] += A[64 x 8] * B[NB x 8]^T per 8 batch rows, where A's rows are output features n (warpgroup g
+// owns features 64 g .. 64 g + 63; rows >= N stay zero), B's rows the K input features plus one row of ones (its column of
+// D is dbias) and zero rows up to the wgmma width NB, and the MMA's reduction dimension is the batch-row index m.  The
+// operands are therefore the TRANSPOSES of the row-major activations; they are transposed on the way into shared memory
+// (each lane owns one batch row of a 32-row slab and writes its elements down a column of the K-major SWIZZLE_128B tile:
+// 32 lanes, 32 distinct banks), split x = hi + lo (both TF32-exact) as in linear_tc.cu, and four products hi*hi + hi*lo +
+// lo*hi + lo*lo accumulate in registers across the CTA's whole row range.  Each CTA writes one partial [N x (K+1)] tile;
+// a second kernel adds the CTAs' partials in CTA order (fixed order -> deterministic).
 #include "common.cuh"
-#include <stdlib.h>
+#include "wgmma_tf32.cuh"
 
 namespace b2r {
 
-constexpr int DW_THREADS = 128;
-constexpr int DW_MROWS = 128;        // UMMA M (A's rows: N valid + zero rows)
 constexpr int DW_SLABS = 2;          // 32-row slabs staged per iteration
-
-__device__ __forceinline__ uint32_t dw_smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
-
-__device__ __forceinline__ uint64_t dw_desc(uint32_t smem_addr) {        // K-major, SWIZZLE_128B (see linear_tc.cu)
-    uint64_t d = 0;
-    d |= (uint64_t)((smem_addr >> 4) & 0x3FFF);
-    d |= (uint64_t)1 << 16;
-    d |= (uint64_t)64 << 32;
-    d |= (uint64_t)1 << 46;
-    d |= (uint64_t)2 << 61;
-    return d;
-}
+constexpr int DW_MAX_WG = 2;         // warpgroups per CTA (N <= 128)
+constexpr int DW_MAX_CTAS_PER_SM = 4;
 
 __device__ __forceinline__ float dw_rn_tf32(float x) { return __uint_as_float((__float_as_uint(x) + 0x1000u) & 0xFFFFE000u); }
 
@@ -40,63 +28,53 @@ __device__ __forceinline__ uint32_t dw_off(int row, int col) {
     return (uint32_t)row * 128u + (uint32_t)((((col >> 2) ^ (row & 7)) << 4) + ((col & 3) << 2));
 }
 
-__global__ void __launch_bounds__(DW_THREADS)
+// blockDim.x = 128 * ceil(N / 64); dynamic shared memory (1024-byte aligned):
+// A_hi[SLABS][64 WG rows * 128B] A_lo[...] B_hi[SLABS][NB * 128B] B_lo[...]
+template <int NB>
+__global__ void __launch_bounds__(128 * DW_MAX_WG)
 k_linear_dw_tc(const float* __restrict__ dY, int lddy, const float* __restrict__ relu_out, const float* __restrict__ X,
-               int ldx, float* __restrict__ part, int M, int N, int K, int rows_per_cta, int tmem_cols) {
+               int ldx, float* __restrict__ part, int M, int N, int K, int rows_per_cta) {
     extern __shared__ __align__(1024) unsigned char dw_raw[];
-    __shared__ __align__(8) uint64_t mma_bar;
-    __shared__ uint32_t tmem_base_sh;
-    const int NB = K + 16;                                      // B's rows: K features, one row of ones, 15 zero rows
-    const size_t a_slab = (size_t)DW_MROWS * 128, b_slab = (size_t)NB * 128;
-    char* A_hi = reinterpret_cast<char*>(dw_raw) + ((1024u - (dw_smem_u32(dw_raw) & 1023u)) & 1023u);
+    const int nwg = blockDim.x / 128, nwarps = blockDim.x / 32;
+    const size_t a_slab = (size_t)nwg * 64 * 128, b_slab = (size_t)NB * 128;
+    char* A_hi = reinterpret_cast<char*>(dw_raw) + ((1024u - (wg_smem_u32(dw_raw) & 1023u)) & 1023u);
     char* A_lo = A_hi + DW_SLABS * a_slab;
     char* B_hi = A_lo + DW_SLABS * a_slab;
     char* B_lo = B_hi + DW_SLABS * b_slab;
-    const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+    const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31, wg = warp >> 2;
 
-    if (warp == 0) {
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(dw_smem_u32(&tmem_base_sh)),
-                     "r"(tmem_cols)
-                     : "memory");
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-    }
-    if (tid == 0) {
-        asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(dw_smem_u32(&mma_bar)), "r"(1) : "memory");
-        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-    }
-    // zero every operand tile once: A's rows N..127, B's rows K+1..K+15 and the lo half of the ones row never change
+    // zero every operand tile once: A's rows N.., B's rows K+1.. and the lo half of the ones row never change
     {
         const size_t total16 = (2 * DW_SLABS * (a_slab + b_slab)) / 16;
         float4* z = reinterpret_cast<float4*>(A_hi);
-        for (size_t i = tid; i < total16; i += DW_THREADS) z[i] = make_float4(0.f, 0.f, 0.f, 0.f);
+        for (size_t i = tid; i < total16; i += blockDim.x) z[i] = make_float4(0.f, 0.f, 0.f, 0.f);
     }
     __syncthreads();
-    for (int e = tid; e < DW_SLABS * 32; e += DW_THREADS)       // the row of ones (hi = 1, lo = 0): row K of B
+    // the row of ones (hi = 1, lo = 0): row K of B.  Batch rows beyond the range have dY = 0 and add nothing to dbias.
+    for (int e = tid; e < DW_SLABS * 32; e += blockDim.x)
         *reinterpret_cast<float*>(B_hi + (e / 32) * b_slab + dw_off(K, e % 32)) = 1.f;
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-    __syncthreads();
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-    const uint32_t tmem = tmem_base_sh;
-    const uint32_t idesc = (1u << 4) | (2u << 7) | (2u << 10) | ((uint32_t)(NB >> 3) << 17) | ((uint32_t)(DW_MROWS >> 4) << 24);
 
+    float acc[NB / 2];
+#pragma unroll
+    for (int i = 0; i < NB / 2; ++i) acc[i] = 0.f;
     const int m_begin = blockIdx.x * rows_per_cta;
     const int m_end = min(M, m_begin + rows_per_cta);
-    uint32_t parity = 0, acc = 0;
+    // staging jobs: (dY | X) x slab; the warps of one job split its features in groups of 32
+    const int job = warp % (2 * DW_SLABS), jpart = warp / (2 * DW_SLABS), jparts = nwarps / (2 * DW_SLABS);
+    const bool isA = job < DW_SLABS;
+    const int slab = job % DW_SLABS;
+    const int nf = isA ? N : K;
+    char* hi = isA ? A_hi + slab * a_slab : B_hi + slab * b_slab;
+    char* lo = isA ? A_lo + slab * a_slab : B_lo + slab * b_slab;
     for (int m0 = m_begin; m0 < m_end; m0 += DW_SLABS * 32) {
-        // warp w stages slab (w % DW_SLABS) of dY (w < DW_SLABS) or X (w >= DW_SLABS): lane = batch row of the slab
+        __syncthreads();                   // every warp's MMAs of the previous iteration completed before the tiles change
         {
-            const bool isA = warp < DW_SLABS;
-            const int s = warp % DW_SLABS;
-            const int m = m0 + s * 32 + lane;
+            const int m = m0 + slab * 32 + lane;
             const bool live = m < m_end;
             const float* src = isA ? dY + (size_t)m * lddy : X + (size_t)m * ldx;
             const float* msk = (isA && relu_out != nullptr) ? relu_out + (size_t)m * lddy : nullptr;
-            char* hi = (isA ? A_hi + s * a_slab : B_hi + s * b_slab);
-            char* lo = (isA ? A_lo + s * a_slab : B_lo + s * b_slab);
-            const int nf = isA ? N : K;
-            // 8 x 128-bit loads (32 features) of the lane's batch row in flight before the first use: the loop is bound by
-            // load latency otherwise (one CTA stages only 64 rows per MMA round)
-            for (int f0 = 0; f0 < nf; f0 += 32) {
+            // 8 x 128-bit loads (32 features) of the lane's batch row in flight before the first use
+            for (int f0 = jpart * 32; f0 < nf; f0 += jparts * 32) {
                 float4 v[8];
 #pragma unroll
                 for (int u = 0; u < 8; ++u) {
@@ -132,323 +110,39 @@ k_linear_dw_tc(const float* __restrict__ dY, int lddy, const float* __restrict__
                     }
                 }
             }
-            if (!isA) {                                              // batch rows beyond the range must not count in dbias
-                *reinterpret_cast<float*>(hi + dw_off(K, lane)) = live ? 1.f : 0.f;
-            }
         }
-        asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-        asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
+        asm volatile("fence.proxy.async.shared::cta;" ::: "memory");      // generic-proxy stores -> async proxy (wgmma)
         __syncthreads();
-        if (tid == 0) {
-            asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-#pragma unroll 1
-            for (int prod = 0; prod < 4; ++prod) {
-                const char* Ab = (prod < 2) ? A_hi : A_lo;           // hi*hi, hi*lo, lo*hi, lo*lo
-                const char* Bb = (prod & 1) ? B_lo : B_hi;
-                for (int s = 0; s < DW_SLABS; ++s) {
+        wg_fence();
 #pragma unroll
-                    for (int k = 0; k < 4; ++k) {                    // 4 MMAs of 8 batch rows (32 bytes) per slab
-                        const uint64_t ad = dw_desc(dw_smem_u32(Ab + s * a_slab) + k * 32);
-                        const uint64_t bd = dw_desc(dw_smem_u32(Bb + s * b_slab) + k * 32);
-                        asm volatile(
-                            "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\t"
-                            "tcgen05.mma.cta_group::1.kind::tf32 [%0], %1, %2, %3, p;\n\t}\n" ::"r"(tmem),
-                            "l"(ad), "l"(bd), "r"(idesc), "r"(acc)
-                            : "memory");
-                        acc = 1;
-                    }
-                }
+        for (int prod = 0; prod < 4; ++prod) {
+            const char* Ab = ((prod < 2) ? A_hi : A_lo) + (size_t)wg * 64 * 128;   // hi*hi, hi*lo, lo*hi, lo*lo
+            const char* Bb = (prod & 1) ? B_lo : B_hi;
+#pragma unroll
+            for (int s = 0; s < DW_SLABS; ++s) {
+#pragma unroll
+                for (int k = 0; k < 4; ++k)                    // 4 MMAs of 8 batch rows (32 bytes) per slab
+                    wgmma_tf32<NB>(acc, wg_desc(wg_smem_u32(Ab + s * a_slab) + k * 32),
+                                   wg_desc(wg_smem_u32(Bb + s * b_slab) + k * 32), 1);
             }
-            asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(
-                             dw_smem_u32(&mma_bar))
-                         : "memory");
         }
-        // bounded wait for the MMAs to have read the tiles (a wrong descriptor must trap, not hang)
-        {
-            const uint32_t addr = dw_smem_u32(&mma_bar);
-            uint32_t done = 0;
-            for (uint32_t spin = 0; spin < (1u << 24) && !done; ++spin) {
-                asm volatile(
-                    "{\n\t.reg .pred p;\n\tmbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n\tselp.u32 %0, 1, 0, p;\n\t}\n"
-                    : "=r"(done)
-                    : "r"(addr), "r"(parity)
-                    : "memory");
-            }
-            if (!done) __trap();
-        }
-        parity ^= 1;
-        acc = 1;                                                     // uniform across threads (only thread 0 uses it)
-        asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
+        wg_commit();
+        wg_wait_all();
+        wg_fence_regs(acc);
     }
-    // epilogue: TMEM lane = output feature n (warps 0..N/32-1 hold the valid lanes), columns 0..K = dW row, column K = dbias
+    // epilogue from the fragment: feature row n, column c of [dW | dbias]
     float* out = part + (size_t)blockIdx.x * N * (K + 1);
-    if (m_begin < m_end) {
-        const int n = warp * 32 + lane;
-        for (int c0 = 0; c0 < NB; c0 += 16) {
-            uint32_t r[16];
-            asm volatile(
-                "tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-                "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];\n"
-                : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-                  "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-                : "r"(tmem + ((uint32_t)(warp * 32) << 16) + (uint32_t)c0));
-            asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-            if (n < N) {
+    const int n0 = wg * 64 + (warp & 3) * 16 + (lane >> 2);
 #pragma unroll
-                for (int i = 0; i < 16; ++i)
-                    if (c0 + i <= K) out[(size_t)n * (K + 1) + c0 + i] = __uint_as_float(r[i]);
+    for (int j = 0; j < NB / 8; ++j) {
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+#pragma unroll
+            for (int c = 0; c < 2; ++c) {
+                const int n = n0 + 8 * h, col = 8 * j + 2 * (lane & 3) + c;
+                if (n < N && col <= K) out[(size_t)n * (K + 1) + col] = acc[4 * j + 2 * h + c];   // 0 for an empty range
             }
         }
-    } else {
-        for (int i = tid; i < N * (K + 1); i += DW_THREADS) out[i] = 0.f;
-    }
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-    __syncthreads();
-    if (warp == 0) {
-        asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem), "r"(tmem_cols) : "memory");
-    }
-}
-
-// ---------------------------------------------------------------------------------------------------------------------
-// Pipelined, stacked version (N <= 64, K <= 112).  Two findings from ncu on the kernel above drive it: (1) it is bound by the
-// latency of its own global loads (18 % issue, 12 % warps active, ~1 TB/s); (2) a kind::tf32 MMA with both operands in shared
-// memory costs ~100 cycles per 32-byte K chunk however narrow its N is (the A-operand read of 128 rows paces it), so three
-// narrow products per chunk waste the tensor pipe.  Here
-//   * the dY / (ReLU mask) / X rows of a 32-row slab travel global -> shared memory as coalesced cp.async copies into a ring
-//     DP_NST slabs deep;
-//   * hi and lo halves are STACKED inside one operand tile each: A = [dY_hi^T (rows 0..63); dY_lo^T (rows 64..127)] uses the
-//     64 rows that were zero padding, B = [X_hi^T, ones, pad (K+16 rows); X_lo^T (K rows)] -- ONE MMA of N = 2K+16 per chunk
-//     produces hi*hi, hi*lo, lo*hi and lo*lo in four blocks of the accumulator, which the epilogue adds;
-//   * the 256 threads transpose + split a landed slab into one of two operand buffers while the MMAs of the previous slab run
-//     out of the other; all slabs of a CTA accumulate into one TMEM tile (one epilogue per CTA, two partial tiles).
-// ---------------------------------------------------------------------------------------------------------------------
-constexpr int DP_THREADS = 512;       // 16 warps: the kernel is bound by per-warp instruction latency with 8
-constexpr int DP_NST = 4;
-constexpr int DP_ITEMS = 6;        // (N + K) * 8 * SLB items per iteration / 512 threads (N + K <= 176, SLB <= 2)
-constexpr int DP_CP = 8;           // 16-byte copies per thread per iteration: 32 * SLB * chunks-per-row / 512
-
-__device__ __forceinline__ void dp_cp16(void* sdst, const void* gsrc, bool valid) {
-    const uint32_t sa = dw_smem_u32(sdst);
-    const int nbytes = valid ? 16 : 0;
-    asm volatile("cp.async.cg.shared.global [%0], [%1], 16, %2;\n" ::"r"(sa), "l"(gsrc), "r"(nbytes) : "memory");
-}
-
-__device__ __forceinline__ void dp_mbar_wait(uint64_t* bar, uint32_t parity) {
-    const uint32_t addr = dw_smem_u32(bar);
-    uint32_t done = 0;
-    for (uint32_t spin = 0; spin < (1u << 24) && !done; ++spin) {
-        asm volatile(
-            "{\n\t.reg .pred p;\n\tmbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n\tselp.u32 %0, 1, 0, p;\n\t}\n"
-            : "=r"(done)
-            : "r"(addr), "r"(parity)
-            : "memory");
-    }
-    if (!done) __trap();
-}
-
-__device__ __forceinline__ void dp_ld16(uint32_t taddr, float (&v)[16]) {
-    uint32_t r[16];
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];\n"
-        : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-          "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-        : "r"(taddr));
-    asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-#pragma unroll
-    for (int i = 0; i < 16; ++i) v[i] = __uint_as_float(r[i]);
-}
-
-// SLB = 32-row slabs per iteration: 2 halves the number of iterations (each costs two block barriers, a proxy fence and an
-// mbarrier round trip: the empty skeleton of the 1-slab loop is 20 us of a 70 us kernel); the masked form keeps 1 (its raw
-// stages are 1.5x larger).
-template <bool MASK, int SLB>
-__global__ void __launch_bounds__(DP_THREADS, 1)
-k_linear_dw_tc_pipe(const float* __restrict__ dY, int lddy, const float* __restrict__ relu_out, const float* __restrict__ X,
-                    int ldx, float* __restrict__ part, int M, int N, int K, int rows_per_cta, int tmem_cols, int ko) {
-    extern __shared__ __align__(1024) unsigned char dw_raw[];
-    __shared__ __align__(8) uint64_t mma_bar[2];
-    __shared__ uint32_t tmem_base_sh;
-    constexpr int NST = SLB == 2 ? 2 : DP_NST;                  // ring depth in iterations
-    constexpr int RPI = 32 * SLB;                               // batch rows per iteration
-    const int NB = K + 16;                                      // B's hi block: K features, the ones row, 15 zero rows
-    const int NB2 = NB + K;                                     // ... followed by the lo block (K rows)
-    const size_t a_slab = (size_t)DW_MROWS * 128, b_slab = (size_t)NB2 * 128;
-    char* ops0 = reinterpret_cast<char*>(dw_raw) + ((1024u - (dw_smem_u32(dw_raw) & 1023u)) & 1023u);
-    const size_t buf_bytes = SLB * (a_slab + b_slab);           // operand buffer: SLB A tiles, then SLB B tiles (b_slab % 1024 == 0)
-    const int segA = N / 4, segM = MASK ? N / 4 : 0, cpr = segA + segM + K / 4;      // 16-byte chunks per raw row
-    const int RS = (cpr + 1) * 4;                                                   // raw row stride in floats (one pad chunk)
-    float* ring = reinterpret_cast<float*>(ops0 + 2 * buf_bytes);
-    const size_t stage_floats = (size_t)RPI * RS;
-    const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-
-    if (warp == 0) {
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(dw_smem_u32(&tmem_base_sh)),
-                     "r"(tmem_cols)
-                     : "memory");
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-    }
-    if (tid == 0) {
-        asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(dw_smem_u32(&mma_bar[0])), "r"(1) : "memory");
-        asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(dw_smem_u32(&mma_bar[1])), "r"(1) : "memory");
-        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-    }
-    const int m_begin = blockIdx.x * rows_per_cta;
-    const int m_end = min(M, m_begin + rows_per_cta);
-    const int nit = m_begin < m_end ? (m_end - m_begin + RPI - 1) / RPI : 0;
-    // copy c of this thread (iteration-invariant): raw row r, source array + column, destination offset in the stage
-    int cp_r[DP_CP], cp_col[DP_CP], cp_dst[DP_CP];              // cp_col: bits 0..1 source (0 dY, 1 mask, 2 X), rest: column
-#pragma unroll
-    for (int i = 0; i < DP_CP; ++i) {
-        const int e = tid + i * DP_THREADS;
-        cp_r[i] = -1; cp_col[i] = 0; cp_dst[i] = 0;
-        if (e < RPI * cpr) {
-            const int r = e / cpr, c = e - r * cpr;
-            cp_r[i] = r;
-            cp_dst[i] = r * RS + c * 4;
-            if (c < segA) cp_col[i] = ((c * 4) << 2) | 0;
-            else if (MASK && c < segA + segM) cp_col[i] = (((c - segA) * 4) << 2) | 1;
-            else cp_col[i] = (((c - segA - segM) * 4) << 2) | 2;
-        }
-    }
-    auto issue_rows = [&](int it, int stage) {
-        if (ko & 8) return;                                  // (diagnostic knock-outs, B2R_TC_KO: 1 MMA, 4 split, 8 loads)
-        float* dst = ring + (size_t)stage * stage_floats;
-        const int m0 = m_begin + it * RPI;
-#pragma unroll
-        for (int i = 0; i < DP_CP; ++i) {
-            if (cp_r[i] < 0) continue;
-            const int m = m0 + cp_r[i];
-            const bool ok = m < m_end;
-            const size_t mm = (size_t)(ok ? m : m_end - 1);
-            const int sel = cp_col[i] & 3, col = cp_col[i] >> 2;
-            const float* src = sel == 0 ? dY + mm * lddy + col : (sel == 1 ? relu_out + mm * lddy + col : X + mm * ldx + col);
-            dp_cp16(dst + cp_dst[i], src, ok);
-        }
-    };
-    for (int s_ = 0; s_ < NST; ++s_) {
-        if (s_ < nit) issue_rows(s_, s_);
-        asm volatile("cp.async.commit_group;\n" ::: "memory");
-    }
-    // zero both operand buffers once: the rows no feature maps to (A: N..63, 64+N..127; B: K+1..K+15) never change
-    {
-        float4* z = reinterpret_cast<float4*>(ops0);
-        for (size_t i = tid; i < 2 * buf_bytes / 16; i += DP_THREADS) z[i] = make_float4(0.f, 0.f, 0.f, 0.f);
-    }
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-    __syncthreads();
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-    const uint32_t tmem = tmem_base_sh;
-    const uint32_t idesc = (1u << 4) | (2u << 7) | (2u << 10) | ((uint32_t)(NB2 >> 3) << 17) | ((uint32_t)(DW_MROWS >> 4) << 24);
-
-    // item i of this thread: (slab sl, feature f, quad of batch rows rq) -> raw offset (floats) and hi / lo chunk offsets
-    // (bytes from the operand buffer's base: A tiles first, then B tiles)
-    int it_raw[DP_ITEMS], it_hi[DP_ITEMS], it_lo[DP_ITEMS];
-    {
-        const int feats = N + K;
-#pragma unroll
-        for (int i = 0; i < DP_ITEMS; ++i) {
-            const int e = tid + i * DP_THREADS;
-            it_raw[i] = -1; it_hi[i] = 0; it_lo[i] = 0;
-            if (e < feats * 8 * SLB) {
-                const int sl = e / (feats * 8), e2 = e - sl * feats * 8;
-                const int f = e2 % feats, rq = e2 / feats;
-                const bool isA = f < N;
-                const int row = isA ? f : f - N, lrow = row + (isA ? 64 : NB);
-                const int tile0 = isA ? sl * (int)a_slab : SLB * (int)a_slab + sl * (int)b_slab;
-                it_raw[i] = (sl * 32 + rq * 4) * RS + (isA ? f : f + segM * 4);   // raw row: [dY | mask | X | pad]
-                it_hi[i] = tile0 + row * 128 + ((rq ^ (row & 7)) << 4);
-                it_lo[i] = tile0 + lrow * 128 + ((rq ^ (lrow & 7)) << 4);
-            }
-        }
-    }
-    for (int it = 0; it < nit; ++it) {
-        const int stage = it % NST, b = it & 1;
-        char* At = ops0 + (size_t)b * buf_bytes;
-        char* Bt = At + SLB * a_slab;
-        asm volatile("cp.async.wait_group %0;\n" ::"n"(NST - 1) : "memory");
-        if (it >= 2) dp_mbar_wait(&mma_bar[b], (uint32_t)(((it >> 1) - 1) & 1));      // MMAs of iteration it-2 have read buffer b
-        __syncthreads();
-        {
-            // transpose on the way: lane = FEATURE (consecutive lanes read consecutive floats of a raw row: conflict-free),
-            // each item takes 4 consecutive batch rows of its feature, splits them, and writes one 16-byte chunk into the
-            // feature's row of the hi block and one into the lo block (the 128B swizzle spreads 8 consecutive rows over the
-            // 8 chunk positions: conflict-free too) -- 4 LDS.32 + 2 STS.128 per 4 elements
-            const float* raw = ring + (size_t)stage * stage_floats;
-#pragma unroll
-            for (int i = 0; i < DP_ITEMS; ++i) {
-                if (it_raw[i] < 0 || (ko & 4)) continue;
-                const float* src = raw + it_raw[i];
-                float x[4] = {src[0], src[RS], src[2 * RS], src[3 * RS]};
-                if (MASK && it_hi[i] < SLB * (int)a_slab) {           // a dY item: apply the ReLU mask
-                    const float* mk = src + N;
-#pragma unroll
-                    for (int j = 0; j < 4; ++j) x[j] = mk[j * RS] > 0.f ? x[j] : 0.f;
-                }
-                float4 h, l;
-                h.x = dw_rn_tf32(x[0]); h.y = dw_rn_tf32(x[1]); h.z = dw_rn_tf32(x[2]); h.w = dw_rn_tf32(x[3]);
-                l.x = dw_rn_tf32(x[0] - h.x); l.y = dw_rn_tf32(x[1] - h.y); l.z = dw_rn_tf32(x[2] - h.z); l.w = dw_rn_tf32(x[3] - h.w);
-                *reinterpret_cast<float4*>(At + it_hi[i]) = h;
-                *reinterpret_cast<float4*>(At + it_lo[i]) = l;
-            }
-            if (warp < SLB)                     // the ones row (dbias): batch rows beyond the range must not count
-                *reinterpret_cast<float*>(Bt + (size_t)warp * b_slab + dw_off(K, lane)) =
-                    (m_begin + it * RPI + warp * 32 + lane < m_end) ? 1.f : 0.f;
-        }
-        asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-        asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-        __syncthreads();
-        if (tid == 0) {
-            asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-#pragma unroll
-            for (int k = 0; k < ((ko & 1) ? 0 : 4 * SLB); ++k) {      // 4 MMAs of 8 batch rows (32 bytes) per slab
-                const uint64_t ad = dw_desc(dw_smem_u32(At + (size_t)(k >> 2) * a_slab) + (k & 3) * 32);
-                const uint64_t bd = dw_desc(dw_smem_u32(Bt + (size_t)(k >> 2) * b_slab) + (k & 3) * 32);
-                const uint32_t acc = (it > 0 || k > 0) ? 1u : 0u;
-                asm volatile(
-                    "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\t"
-                    "tcgen05.mma.cta_group::1.kind::tf32 [%0], %1, %2, %3, p;\n\t}\n" ::"r"(tmem),
-                    "l"(ad), "l"(bd), "r"(idesc), "r"(acc)
-                    : "memory");
-            }
-            asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(
-                             dw_smem_u32(&mma_bar[b]))
-                         : "memory");
-        }
-        if (it + NST < nit) issue_rows(it + NST, stage);              // every thread is past its reads of this ring stage
-        asm volatile("cp.async.commit_group;\n" ::: "memory");
-    }
-    asm volatile("cp.async.wait_group 0;\n" ::: "memory");
-    // two partial tiles per CTA: tile 0 = (hi*hi + hi*lo) from accumulator rows 0..63, tile 1 = (lo*hi + lo*lo) from rows 64..127
-    const int T = N * (K + 1);
-    const int q = warp & 3;
-    float* out = part + ((size_t)2 * blockIdx.x + (q >> 1)) * T;
-    if (nit > 0) {
-        dp_mbar_wait(&mma_bar[(nit - 1) & 1], (uint32_t)(((nit - 1) >> 1) & 1));    // the last commit covers every MMA before it
-        asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-        const int n = (q & 1) * 32 + lane;
-        const uint32_t lane_base = tmem + ((uint32_t)(q * 32) << 16);
-        for (int c0 = (warp >> 2) * 16; c0 < NB; c0 += 16 * (DP_THREADS / 128)) {
-            float v[16], w[16];
-            dp_ld16(lane_base + (uint32_t)c0, v);
-            if (c0 < K) {                                            // the X_lo block's columns NB + c0 .. +15
-                dp_ld16(lane_base + (uint32_t)(NB + c0), w);
-#pragma unroll
-                for (int i = 0; i < 16; ++i) v[i] += w[i];
-            }
-            if (n < N) {
-#pragma unroll
-                for (int i = 0; i < 16; ++i)
-                    if (c0 + i <= K) out[(size_t)n * (K + 1) + c0 + i] = v[i];
-            }
-        }
-    } else {
-        for (int i = tid; i < 2 * T; i += DP_THREADS) part[(size_t)2 * blockIdx.x * T + i] = 0.f;
-    }
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-    __syncthreads();
-    if (warp == 0) {
-        asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem), "r"(tmem_cols) : "memory");
     }
 }
 
@@ -474,11 +168,26 @@ k_linear_dw_reduce(const float* __restrict__ part, int ctas, int N, int K, float
     }
 }
 
-static int dw_ctas(int64_t M) {
-    int64_t slabs = (M + DW_SLABS * 32 - 1) / (DW_SLABS * 32);
-    int64_t c = (int64_t)sm_count() * 2;
-    if (c > slabs) c = slabs;
-    return (int)(c < 1 ? 1 : c);
+template <int NB>
+static int launch_linear_dw_tc(const float* dY, int lddy, const float* relu_out, const float* X, int ldx, float* dW,
+                               float* dbias, int M, int N, int K, float* part, cudaStream_t s) {
+    const int nwg = (N + 63) / 64;
+    const size_t smem = (size_t)2 * DW_SLABS * nwg * 64 * 128 + (size_t)2 * DW_SLABS * NB * 128 + 1024;
+    B2R_CUDA_OK(cudaFuncSetAttribute(k_linear_dw_tc<NB>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    int per_sm = 0;
+    B2R_CUDA_OK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_linear_dw_tc<NB>, 128 * nwg, smem));
+    if (per_sm > DW_MAX_CTAS_PER_SM) per_sm = DW_MAX_CTAS_PER_SM;
+    if (per_sm < 1) per_sm = 1;
+    const int64_t slabs = ((int64_t)M + DW_SLABS * 32 - 1) / (DW_SLABS * 32);
+    int ctas = sm_count() * per_sm;
+    if (ctas > slabs) ctas = (int)slabs;
+    const int rows_per_cta = (int)((slabs + ctas - 1) / ctas) * DW_SLABS * 32;
+    k_linear_dw_tc<NB><<<ctas, 128 * nwg, smem, s>>>(dY, lddy, relu_out, X, ldx, part, M, N, K, rows_per_cta);
+    B2R_LAUNCH_OK("k_linear_dw_tc");
+    const int total = N * (K + 1);
+    k_linear_dw_reduce<<<(total + 31) / 32, 256, 0, s>>>(part, ctas, N, K, dW, dbias);
+    B2R_LAUNCH_OK("k_linear_dw_reduce");
+    return 0;
 }
 
 }  // namespace b2r
@@ -487,8 +196,8 @@ using namespace b2r;
 
 extern "C" size_t b2r_linear_bwd_weight_tc_workspace_bytes(int64_t M, int N, int K) {
     if (M <= 0 || N <= 0 || K <= 0) return 0;
-    // partial tiles: the first kernel writes one per CTA (<= 2 per SM), the pipelined one two per CTA (1 CTA per SM)
-    return align_up((size_t)2 * sm_count() * N * (K + 1) * 4, 256);
+    // one partial tile per CTA, at most DW_MAX_CTAS_PER_SM CTAs per SM
+    return align_up((size_t)DW_MAX_CTAS_PER_SM * sm_count() * N * (K + 1) * 4, 256);
 }
 
 // returns B2R_E_UNSUPPORTED for shapes outside the tensor-core kernel's class (callers fall back to b2r_linear_bwd_weight)
@@ -496,66 +205,17 @@ extern "C" int b2r_linear_bwd_weight_tc(const float* dY, int lddy, const float* 
                                         float* dbias, int64_t M, int N, int K, void* ws, size_t ws_bytes,
                                         b2r_stream_t stream) {
     B2R_REQUIRE(dY && X && dW && ws, B2R_E_BADARG, "b2r_linear_bwd_weight_tc: null pointer");
-    if (!(N % 4 == 0 && N >= 4 && N <= 128 && K % 16 == 0 && K >= 16 && K <= 240 && M > 0 && M <= 0x7fffffff &&
-          lddy % 4 == 0 && ldx % 4 == 0 && lddy >= N && ldx >= K && aligned16(dY) && aligned16(X) &&
+    if (!(N % 4 == 0 && N >= 4 && N <= 64 * DW_MAX_WG && K % 16 == 0 && K >= 16 && K <= 240 && M > 0 &&
+          M <= 0x7fffffff && lddy % 4 == 0 && ldx % 4 == 0 && lddy >= N && ldx >= K && aligned16(dY) && aligned16(X) &&
           (relu_out == nullptr || aligned16(relu_out))))
         return set_error(B2R_E_UNSUPPORTED, "b2r_linear_bwd_weight_tc: shape M=%lld N=%d K=%d outside the kernel's class",
                          (long long)M, N, K);
     B2R_REQUIRE(ws_bytes >= b2r_linear_bwd_weight_tc_workspace_bytes(M, N, K), B2R_E_WORKSPACE,
                 "b2r_linear_bwd_weight_tc: workspace too small");
-    int cols = 32;
-    while (cols < K + 16) cols <<= 1;
     cudaStream_t s = as_stream(stream);
     float* part = static_cast<float*>(ws);
-    {   // pipelined kernel with stacked hi/lo operand tiles when the shape allows and its shared memory fits
-        static const bool use_pipe = !(getenv("B2R_TC_PIPE") && atoi(getenv("B2R_TC_PIPE")) == 0);
-        static const int ko = getenv("B2R_TC_KO") ? atoi(getenv("B2R_TC_KO")) : 0;     // diagnostic: wrong results by design
-        static const int want_slb = getenv("B2R_DW_SLB") ? atoi(getenv("B2R_DW_SLB")) : 2;
-        const int cpr = N / 4 + (relu_out ? N / 4 : 0) + K / 4;
-        const int NB2 = 2 * K + 16;
-        const size_t tiles = (size_t)DW_MROWS * 128 + (size_t)NB2 * 128;
-        const size_t lim = 227 * 1024 - 64;
-        auto need = [&](int slb) { return 2 * slb * tiles + (size_t)(slb == 2 ? 2 : DP_NST) * 32 * slb * (cpr + 1) * 16 + 1024; };
-        int slb = (!relu_out && want_slb == 2 && need(2) <= lim && 64 * cpr <= DP_CP * DP_THREADS) ? 2 : 1;
-        const size_t psmem = need(slb);
-        if (use_pipe && N <= 64 && NB2 <= 256 && (N + K) * 8 * slb <= DP_ITEMS * DP_THREADS && 32 * slb * cpr <= DP_CP * DP_THREADS &&
-            psmem <= lim) {
-            int pcols = 32;
-            while (pcols < NB2) pcols <<= 1;
-            const int rpi = 32 * slb;
-            const int64_t units = (M + rpi - 1) / rpi;
-            int ctas = sm_count();
-            if (ctas > units) ctas = (int)units;
-            const int rows_per_cta = (int)((units + ctas - 1) / ctas) * rpi;
-#define B2R_DP(MK, SL)                                                                                          \
-    do {                                                                                                        \
-        B2R_CUDA_OK(cudaFuncSetAttribute(k_linear_dw_tc_pipe<MK, SL>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)psmem)); \
-        k_linear_dw_tc_pipe<MK, SL><<<ctas, DP_THREADS, psmem, s>>>(dY, lddy, relu_out, X, ldx, part, (int)M, N, K, rows_per_cta, \
-                                                                   pcols, ko);                                \
-    } while (0)
-            if (relu_out) B2R_DP(true, 1); else if (slb == 2) B2R_DP(false, 2); else B2R_DP(false, 1);
-#undef B2R_DP
-            B2R_LAUNCH_OK("k_linear_dw_tc_pipe");
-            const int total = N * (K + 1);
-            k_linear_dw_reduce<<<(total + 31) / 32, 256, 0, s>>>(part, 2 * ctas, N, K, dW, dbias);
-            B2R_LAUNCH_OK("k_linear_dw_reduce");
-            return 0;
-        }
-    }
-    const size_t smem = (size_t)2 * DW_SLABS * DW_MROWS * 128 + (size_t)2 * DW_SLABS * (K + 16) * 128 + 1024;
-    if (smem > 200 * 1024) return set_error(B2R_E_UNSUPPORTED, "b2r_linear_bwd_weight_tc: %zu B of shared memory needed", smem);
-    const int ctas = dw_ctas(M);
-    const int64_t slabs = (M + DW_SLABS * 32 - 1) / (DW_SLABS * 32);
-    const int rows_per_cta = (int)((slabs + ctas - 1) / ctas) * DW_SLABS * 32;
-    static size_t attr = 0;
-    if (smem > attr) {
-        B2R_CUDA_OK(cudaFuncSetAttribute(k_linear_dw_tc, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        attr = smem;
-    }
-    k_linear_dw_tc<<<ctas, DW_THREADS, smem, s>>>(dY, lddy, relu_out, X, ldx, part, (int)M, N, K, rows_per_cta, cols);
-    B2R_LAUNCH_OK("k_linear_dw_tc");
-    const int total = N * (K + 1);
-    k_linear_dw_reduce<<<(total + 31) / 32, 256, 0, s>>>(part, ctas, N, K, dW, dbias);
-    B2R_LAUNCH_OK("k_linear_dw_reduce");
-    return 0;
+    // wgmma width: K features + the ones row, rounded up to the instantiated widths
+    if (K + 1 <= 48) return launch_linear_dw_tc<48>(dY, lddy, relu_out, X, ldx, dW, dbias, (int)M, N, K, part, s);
+    if (K + 1 <= 80) return launch_linear_dw_tc<80>(dY, lddy, relu_out, X, ldx, dW, dbias, (int)M, N, K, part, s);
+    return launch_linear_dw_tc<256>(dY, lddy, relu_out, X, ldx, dW, dbias, (int)M, N, K, part, s);
 }

@@ -1,92 +1,27 @@
-// linear_tc.cu -- nn.Linear forward on the 5th-generation tensor cores (tcgen05.mma kind::tf32, accumulator in TMEM)
-// with fp32-class accuracy: every operand is split x = hi + lo (hi = the TF32 truncation the hardware would apply
-// anyway, lo = the exact remainder) and four products hi*hi + hi*lo + lo*hi + lo*lo are accumulated in the same
-// TMEM tile, which brings the result to ~2^-21 relative of the fp32 answer (the 1e-5 parity bar of the north star
-// rules out a single TF32 product at trained-scale weights, SURVEY.md 7.3.4).
+// linear_tc.cu -- nn.Linear forward on the Hopper tensor cores (wgmma.mma_async, TF32 operands, fp32 accumulator in
+// registers) with fp32-class accuracy: every operand is split x = hi + lo (hi = x rounded to TF32, lo = the TF32 rounding of
+// the remainder) and three products hi*hi + hi*lo + lo*hi are accumulated in the same registers, which brings the result to
+// ~2^-21 relative of the fp32 answer (the 1e-5 parity bar rules out a single TF32 product at trained-scale weights,
+// SURVEY.md 7.3.4).
 //
 // Shape class: the q/k/v and feed-forward Linear layers of utils/layers.py:26-28,106-107 and NeuMF's tower
 // (NeuMF.py:70): Y[M,N] = act(X[M,K] W^T + b) with small K (multiple of 32 floats, <= 128) and N (multiple of 16,
-// <= 256) and M = B*L in the hundreds of thousands -- each CTA owns 128-row tiles of X, W stays resident in shared
-// memory for the CTA's lifetime, so the kernel streams X once and Y once (HBM-bound) while the MMAs ride along.
+// <= 256) and M = B*L in the hundreds of thousands -- each CTA (one warpgroup) owns 64-row tiles of X, W stays resident
+// in shared memory for the CTA's lifetime, so the kernel streams X once and Y once (HBM-bound) while the MMAs ride along.
 //
-// Operand staging: no TMA.  Threads load X / W with coalesced 128-bit loads, split hi/lo in registers and store both
-// halves into shared memory in the canonical K-major SWIZZLE_128B layout the UMMA descriptor expects (one 128-byte
-// row = 32 floats of K; 16-byte chunk index XOR (row & 7); 8-row groups 1024 bytes apart), then
-// fence.proxy.async + barrier, and ONE thread issues the 4*(K/8) MMAs and commits them to an mbarrier.  The epilogue
-// reads the accumulator back with tcgen05.ld (32 lanes x 16 columns per instruction), adds the bias, applies ReLU and
-// writes Y.
+// Operand staging: threads load X / W with coalesced 128-bit loads, split hi/lo in registers and store both halves into
+// shared memory in the K-major SWIZZLE_128B layout of wgmma_tf32.cuh, then fence.proxy.async + barrier, and the
+// warpgroup issues 3 * (K / 8) wgmmas.  The loads of the CTA's next tile are issued before the MMA wait, so they stay in
+// flight through the MMAs and the epilogue, which adds the bias, applies ReLU and stores Y straight from the accumulator.
 #include "common.cuh"
-#include <stdlib.h>
+#include "wgmma_tf32.cuh"
 
 namespace b2r {
 
-constexpr int TC_M = 128;          // rows per tile == UMMA M
-constexpr int TC_THREADS = 128;    // 4 warps: warp w reads TMEM lanes [32w, 32w+32)
+constexpr int TC_M = 64;           // rows per tile == wgmma M
+constexpr int TC_THREADS = 128;    // one warpgroup
 
-__device__ __forceinline__ uint32_t tc_smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
-
-__device__ __forceinline__ uint64_t tc_desc(uint32_t smem_addr) {
-    // K-major, SWIZZLE_128B: start address >> 4 in [0,14); LBO (ignored for swizzled K-major) = 1 in [16,30);
-    // SBO = 1024 B >> 4 = 64 in [32,46); descriptor version 1 (Blackwell) in [46,48); layout type 2 in [61,64)
-    uint64_t d = 0;
-    d |= (uint64_t)((smem_addr >> 4) & 0x3FFF);
-    d |= (uint64_t)1 << 16;
-    d |= (uint64_t)64 << 32;
-    d |= (uint64_t)1 << 46;
-    d |= (uint64_t)2 << 61;
-    return d;
-}
-
-__device__ __forceinline__ void tc_mma_tf32(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t acc) {
-    asm volatile(
-        "{\n\t"
-        ".reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::tf32 [%0], %1, %2, %3, p;\n\t"
-        "}\n" ::"r"(tmem_d), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(acc)
-        : "memory");
-}
-
-__device__ __forceinline__ void tc_commit(uint64_t* bar) {
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(tc_smem_u32(bar))
-                 : "memory");
-}
-
-__device__ __forceinline__ void tc_mbar_init(uint64_t* bar, int count) {
-    asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(tc_smem_u32(bar)), "r"(count) : "memory");
-}
-
-// bounded wait: a wrong descriptor must end in a trap, not in a hung GPU
-__device__ __forceinline__ void tc_mbar_wait(uint64_t* bar, uint32_t parity) {
-    const uint32_t addr = tc_smem_u32(bar);
-    for (uint32_t spin = 0; spin < (1u << 24); ++spin) {
-        uint32_t done;
-        asm volatile(
-            "{\n\t.reg .pred p;\n\t"
-            "mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n\t"
-            "selp.u32 %0, 1, 0, p;\n\t}\n"
-            : "=r"(done)
-            : "r"(addr), "r"(parity)
-            : "memory");
-        if (done) return;
-    }
-    __trap();
-}
-
-__device__ __forceinline__ void tc_ld16(uint32_t taddr, float (&v)[16]) {
-    uint32_t r[16];
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];\n"
-        : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-          "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-        : "r"(taddr));
-    asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-#pragma unroll
-    for (int i = 0; i < 16; ++i) v[i] = __uint_as_float(r[i]);
-}
-
-// round to the nearest TF32 value (10 explicit mantissa bits): the hardware truncates the low 13 bits of what it is
+// round to the nearest TF32 value (10 explicit mantissa bits): the tensor core ignores the low 13 bits of what it is
 // given, so operands are pre-rounded here and arrive exactly representable
 __device__ __forceinline__ float tc_rn_tf32(float x) { return __uint_as_float((__float_as_uint(x) + 0x1000u) & 0xFFFFE000u); }
 
@@ -101,343 +36,132 @@ __device__ __forceinline__ void tc_store_split(char* hi_base, char* lo_base, int
     *reinterpret_cast<float4*>(lo_base + off) = l;
 }
 
-// dynamic shared memory (1024-byte aligned): A_hi[KS][128*128B] A_lo[...] B_hi[KS][N*128B] B_lo[...]
-template <int KS>
+// dynamic shared memory (1024-byte aligned): A_hi[KS][64*128B] A_lo[...] B_hi[KS][NW*128B] B_lo[...]; NW >= N is the
+// wgmma width, W's rows N..NW-1 are zero and their output columns are not stored
+template <int KS, int NW>
 __global__ void __launch_bounds__(TC_THREADS)
-k_linear_fwd_tc(const float* __restrict__ X, int ldx, const float* __restrict__ amask, const float* __restrict__ W,
-                const float* __restrict__ bias, float* __restrict__ Y, int ldy, int M, int N, int relu, int tmem_cols, int nprod) {
+k_linear_tc(const float* __restrict__ X, int ldx, const float* __restrict__ amask, const float* __restrict__ W,
+            const float* __restrict__ bias, float* __restrict__ Y, int ldy, int M, int N, int relu) {
     extern __shared__ __align__(1024) unsigned char smem_raw[];
-    __shared__ __align__(8) uint64_t mma_bar;
-    __shared__ uint32_t tmem_base_sh;
     constexpr int K = KS * 32;                              // KS 128-byte K slabs
-    const size_t a_slab = (size_t)TC_M * 128, b_slab = (size_t)N * 128;
+    constexpr int LPT = 8 * KS * TC_M / TC_THREADS;         // 16-byte loads per thread per tile
+    constexpr size_t a_slab = (size_t)TC_M * 128, b_slab = (size_t)NW * 128;
     // swizzle-128B operand tiles need 1024-byte aligned bases: align by hand (the launch adds 1 KB of slack)
-    char* A_hi = reinterpret_cast<char*>(smem_raw) + ((1024u - (tc_smem_u32(smem_raw) & 1023u)) & 1023u);
+    char* A_hi = reinterpret_cast<char*>(smem_raw) + ((1024u - (wg_smem_u32(smem_raw) & 1023u)) & 1023u);
     char* A_lo = A_hi + KS * a_slab;
     char* B_hi = A_lo + KS * a_slab;
     char* B_lo = B_hi + KS * b_slab;
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
 
-    if (warp == 0) {
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(tc_smem_u32(&tmem_base_sh)),
-                     "r"(tmem_cols)
-                     : "memory");
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-    }
-    if (tid == 0) {
-        tc_mbar_init(&mma_bar, 1);
-        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-    }
     // W -> B_hi / B_lo (once per CTA): element (n, slab s, chunk c) <- W[n*K + s*32 + c*4 ..]
-    for (int e = tid; e < N * KS * 8; e += TC_THREADS) {
+    for (int e = tid; e < NW * KS * 8; e += TC_THREADS) {
         const int c = e % 8, s = (e / 8) % KS, n = e / (8 * KS);
-        const float4 v = *reinterpret_cast<const float4*>(W + (size_t)n * K + s * 32 + c * 4);
+        const float4 v = n < N ? *reinterpret_cast<const float4*>(W + (size_t)n * K + s * 32 + c * 4)
+                               : make_float4(0.f, 0.f, 0.f, 0.f);
         tc_store_split(B_hi + s * b_slab, B_lo + s * b_slab, n, c, v);
     }
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-    __syncthreads();
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-    const uint32_t tmem = tmem_base_sh;
-    const uint32_t idesc = (1u << 4) | (2u << 7) | (2u << 10) | ((uint32_t)(N >> 3) << 17) | ((uint32_t)(TC_M >> 4) << 24);
 
-    uint32_t parity = 0;
     const int ntiles = (M + TC_M - 1) / TC_M;
-    // Software pipeline over this CTA's tiles: the 8*KS 128-bit loads of the NEXT tile are issued right after this tile's
-    // MMAs and stay in flight through the MMA wait and the epilogue; shared memory and the TMEM accumulator are single
-    // buffers (the mbarrier wait orders "MMAs done" before both are reused), several CTAs per SM cover the rest.
-    float4 v[8 * KS];
-#define TC_ISSUE_LOADS(TILE)                                                                         \
-    do {                                                                                             \
-        const int m0_ = (TILE) * TC_M;                                                               \
-        _Pragma("unroll") for (int i = 0; i < 8 * KS; ++i) {                                         \
-            const int e = i * TC_THREADS + tid;                                                      \
-            const int c = e % 8, s_ = (e / 8) % KS, r = e / (8 * KS);                                \
-            v[i] = make_float4(0.f, 0.f, 0.f, 0.f);                                                  \
-            if (m0_ + r < M) {                                                                       \
-                const size_t g = (size_t)(m0_ + r) * ldx + s_ * 32 + c * 4;                          \
-                v[i] = ld_row4(X + g);                                                               \
-                if (amask != nullptr) {      /* ReLU backward: keep dY where the saved output > 0 */ \
-                    const float4 mk = ld_row4(amask + g);                                            \
-                    v[i].x = mk.x > 0.f ? v[i].x : 0.f;                                              \
-                    v[i].y = mk.y > 0.f ? v[i].y : 0.f;                                              \
-                    v[i].z = mk.z > 0.f ? v[i].z : 0.f;                                              \
-                    v[i].w = mk.w > 0.f ? v[i].w : 0.f;                                              \
-                }                                                                                    \
-            }                                                                                        \
-        }                                                                                            \
-    } while (0)
+    float4 v[LPT];
+    auto issue_loads = [&](int tile) {
+        const int m0 = tile * TC_M;
+#pragma unroll
+        for (int i = 0; i < LPT; ++i) {
+            const int e = i * TC_THREADS + tid;
+            const int c = e % 8, s = (e / 8) % KS, r = e / (8 * KS);
+            v[i] = make_float4(0.f, 0.f, 0.f, 0.f);
+            if (m0 + r < M) {
+                const size_t g = (size_t)(m0 + r) * ldx + s * 32 + c * 4;
+                v[i] = ld_row4(X + g);
+                if (amask != nullptr) {      // ReLU backward: keep dY where the saved output > 0
+                    const float4 mk = ld_row4(amask + g);
+                    v[i].x = mk.x > 0.f ? v[i].x : 0.f;
+                    v[i].y = mk.y > 0.f ? v[i].y : 0.f;
+                    v[i].z = mk.z > 0.f ? v[i].z : 0.f;
+                    v[i].w = mk.w > 0.f ? v[i].w : 0.f;
+                }
+            }
+        }
+    };
+    float acc[NW / 2];
+#pragma unroll
+    for (int i = 0; i < NW / 2; ++i) acc[i] = 0.f;
     int tile = blockIdx.x;
-    if (tile < ntiles) TC_ISSUE_LOADS(tile);
+    if (tile < ntiles) issue_loads(tile);
     for (; tile < ntiles; tile += gridDim.x) {
         const int m0 = tile * TC_M;
+        __syncthreads();                  // the previous tile's MMAs have completed in every warp before A is overwritten
 #pragma unroll
-        for (int i = 0; i < 8 * KS; ++i) {
+        for (int i = 0; i < LPT; ++i) {
             const int e = i * TC_THREADS + tid;
-            const int c = e % 8, s_ = (e / 8) % KS, r = e / (8 * KS);
-            tc_store_split(A_hi + s_ * a_slab, A_lo + s_ * a_slab, r, c, v[i]);
+            const int c = e % 8, s = (e / 8) % KS, r = e / (8 * KS);
+            tc_store_split(A_hi + s * a_slab, A_lo + s * a_slab, r, c, v[i]);
         }
-        asm volatile("fence.proxy.async.shared::cta;" ::: "memory");      // generic-proxy stores -> async proxy (UMMA)
-        asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-        __syncthreads();                  // also: every thread's tcgen05.ld of the previous tile has completed (wait::ld)
-        if (tid == 0) {
-            asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-            uint32_t acc = 0;
-#pragma unroll 1
-            for (int prod = 0; prod < nprod; ++prod) {
-                const char* Ab = (prod < 2) ? A_hi : A_lo;              // hi*hi, hi*lo, lo*hi [, lo*lo]
-                const char* Bb = (prod & 1) ? B_lo : B_hi;
-                for (int s_ = 0; s_ < KS; ++s_) {
-#pragma unroll
-                    for (int k = 0; k < 4; ++k) {                       // 4 MMAs of K = 8 floats (32 bytes) per slab
-                        const uint64_t ad = tc_desc(tc_smem_u32(Ab + s_ * a_slab) + k * 32);
-                        const uint64_t bd = tc_desc(tc_smem_u32(Bb + s_ * b_slab) + k * 32);
-                        tc_mma_tf32(tmem, ad, bd, idesc, acc);
-                        acc = 1;
-                    }
-                }
-            }
-            tc_commit(&mma_bar);
-        }
-        if (tile + (int)gridDim.x < ntiles) TC_ISSUE_LOADS(tile + (int)gridDim.x);
-        tc_mbar_wait(&mma_bar, parity);
-        parity ^= 1;
-        asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-        // epilogue: thread = row (TMEM lane), 16 columns per tcgen05.ld
-        const int row = m0 + warp * 32 + lane;
-        for (int c0 = 0; c0 < N; c0 += 16) {
-            float y16[16];
-            tc_ld16(tmem + ((uint32_t)(warp * 32) << 16) + (uint32_t)c0, y16);
-            if (row < M) {
-#pragma unroll
-                for (int i = 0; i < 16; ++i) {
-                    float y = y16[i] + (bias != nullptr ? bias[c0 + i] : 0.f);
-                    if (relu) y = fmaxf(y, 0.f);
-                    y16[i] = y;
-                }
-                float* dst = Y + (size_t)row * ldy + c0;
-#pragma unroll
-                for (int i = 0; i < 16; i += 4) *reinterpret_cast<float4*>(dst + i) = make_float4(y16[i], y16[i + 1], y16[i + 2], y16[i + 3]);
-            }
-        }
-    }
-#undef TC_ISSUE_LOADS
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-    __syncthreads();
-    if (warp == 0) {
-        asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem), "r"(tmem_cols) : "memory");
-    }
-}
-
-
-// ---------------------------------------------------------------------------------------------------------------------
-// Pipelined version (K <= 64): the kernel above keeps 8 warps per SM and is bound by the latency of its own loads (ncu:
-// 11 % issue, 12 % warps active, 1.2 TB/s).  Here the X tiles (and the ReLU mask tiles) travel global -> shared memory as
-// cp.async 16-byte copies into a ring that is NST tiles deep, so 64-96 KB per SM are always in flight; the 256 threads
-// split a landed raw tile into the swizzled hi / lo operand tiles, one thread issues the MMAs into one of TWO TMEM
-// accumulators, and the epilogue of tile i-1 (tcgen05.ld, bias, ReLU, stores) runs while the MMAs of tile i execute.
-//   iteration i:  wait(raw tile i landed) ; wait(MMA i-1 done: hi/lo free) ; split ; MMA i -> acc[i&1] ; refill ring with
-//                 tile i+NST ; epilogue i-1 from acc[(i-1)&1]
-// ---------------------------------------------------------------------------------------------------------------------
-// 16 warps: with 8, each scheduler holds 2 warps and the kernel is bound by per-warp instruction latency (ncu: 20 % issue
-// slots, stalls spread over the split / epilogue chains) rather than by HBM, the tensor pipe or the ring depth
-constexpr int TP_THREADS = 512;
-
-__device__ __forceinline__ void tp_cp16(void* sdst, const void* gsrc, bool valid) {
-    const uint32_t sa = tc_smem_u32(sdst);
-    const int nbytes = valid ? 16 : 0;                       // src-size 0: writes zeros, reads nothing
-    asm volatile("cp.async.cg.shared.global [%0], [%1], 16, %2;\n" ::"r"(sa), "l"(gsrc), "r"(nbytes) : "memory");
-}
-
-template <int KS, bool MASK, bool DB>
-__global__ void __launch_bounds__(TP_THREADS, 1)
-k_linear_tc_pipe(const float* __restrict__ X, int ldx, const float* __restrict__ amask, const float* __restrict__ W,
-                 const float* __restrict__ bias, float* __restrict__ Y, int ldy, int M, int N, int relu, int acc_cols,
-                 int nprod, int ko, int ystage_lg) {
-    extern __shared__ __align__(1024) unsigned char smem_raw[];
-    __shared__ __align__(8) uint64_t mma_bar[2];
-    __shared__ uint32_t tmem_base_sh;
-    constexpr int K = KS * 32;
-    // DB: two hi/lo operand buffers -- the split of tile i+1 runs while the MMAs of tile i execute (the tensor pipe, at
-    // ~2 cycles per accumulator column per 32-byte K chunk for kind::tf32, is the longest stage of a tile); the ring is then
-    // two tiles deep to stay inside 227 KB.  The masked form keeps one buffer (its ring stages are two raw tiles each).
-    constexpr int NST = (MASK || DB) ? 2 : 3;                // ring depth
-    constexpr int CH = TC_M * K / 4;                         // 16-byte chunks per raw tile
-    constexpr int CPT = CH / TP_THREADS;                     // chunks per thread
-    const size_t a_slab = (size_t)TC_M * 128, b_slab = (size_t)N * 128, raw_tile = (size_t)TC_M * K * 4;
-    char* A_hi = reinterpret_cast<char*>(smem_raw) + ((1024u - (tc_smem_u32(smem_raw) & 1023u)) & 1023u);
-    constexpr int NBUF = DB ? 2 : 1;
-    const size_t ab_bytes = 2 * KS * a_slab;                 // one operand buffer: A_hi slabs, then A_lo slabs
-    char* B_hi = A_hi + NBUF * ab_bytes;
-    char* B_lo = B_hi + KS * b_slab;
-    char* ring = B_lo + KS * b_slab;                         // NST x (raw X tile [, raw mask tile])
-    const size_t stage_bytes = raw_tile * (MASK ? 2 : 1);
-    // output staging tile [128][N] (ystage_lg >= 0: N / 4 = 2^ystage_lg chunks per row, chunk index XOR (row & (N/4 - 1))):
-    // the accumulator comes out of TMEM one ROW per lane, and 16-byte stores at a 4N-byte lane stride cost a third of the
-    // kernel (knock-out measurement); through this tile the global stores are full rows
-    char* ystage = ring + NST * stage_bytes;
-    const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-
-    if (warp == 0) {
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(tc_smem_u32(&tmem_base_sh)),
-                     "r"(2 * acc_cols)
-                     : "memory");
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-    }
-    if (tid == 0) {
-        tc_mbar_init(&mma_bar[0], 1);
-        tc_mbar_init(&mma_bar[1], 1);
-        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-    }
-    const int ntiles = (M + TC_M - 1) / TC_M;
-    // ring prologue: tiles 0 .. NST-1 of this CTA
-    auto issue_tile = [&](int tile, int stage) {
-        if (ko & 8) return;                                  // (diagnostic knock-outs, B2R_TC_KO: 1 MMA, 2 stores, 4 split, 8 loads)
-        char* dst = ring + (size_t)stage * stage_bytes;
-        const int m0 = tile * TC_M;
-#pragma unroll
-        for (int i = 0; i < CPT; ++i) {
-            const int e = i * TP_THREADS + tid;
-            const int r = e / (K / 4), c = e % (K / 4);
-            const bool ok = m0 + r < M;
-            const size_t g = (size_t)(ok ? m0 + r : M - 1) * ldx + c * 4;
-            tp_cp16(dst + (size_t)e * 16, X + g, ok);
-            if (MASK) tp_cp16(dst + raw_tile + (size_t)e * 16, amask + g, ok);
-        }
-    };
-#pragma unroll
-    for (int s_ = 0; s_ < NST; ++s_) {
-        const int t = blockIdx.x + s_ * gridDim.x;
-        if (t < ntiles) issue_tile(t, s_);
-        asm volatile("cp.async.commit_group;\n" ::: "memory");
-    }
-    // W -> B_hi / B_lo (once per CTA)
-    for (int e = tid; e < N * KS * 8; e += TP_THREADS) {
-        const int c = e % 8, s_ = (e / 8) % KS, n = e / (8 * KS);
-        const float4 v = *reinterpret_cast<const float4*>(W + (size_t)n * K + s_ * 32 + c * 4);
-        tc_store_split(B_hi + s_ * b_slab, B_lo + s_ * b_slab, n, c, v);
-    }
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-    __syncthreads();
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-    const uint32_t tmem = tmem_base_sh;
-    const uint32_t idesc = (1u << 4) | (2u << 7) | (2u << 10) | ((uint32_t)(N >> 3) << 17) | ((uint32_t)(TC_M >> 4) << 24);
-
-    // epilogue of one finished tile: warp w reads TMEM lanes [32 (w & 3), +32) and the 16-column chunks (w >> 2), (w >> 2) + 4, ...
-    auto epilogue = [&](int tile, uint32_t acc_base) {
-        const int row_l = (warp & 3) * 32 + lane;
-        const int row = tile * TC_M + row_l;
-        const int ncm = (1 << (ystage_lg < 0 ? 0 : ystage_lg)) - 1;
-        for (int c0 = (warp >> 2) * 16; c0 < N; c0 += 16 * (TP_THREADS / 128)) {
-            float y16[16];
-            tc_ld16(acc_base + ((uint32_t)((warp & 3) * 32) << 16) + (uint32_t)c0, y16);
-            if ((row < M || ystage_lg >= 0) && !(ko & 2)) {
-#pragma unroll
-                for (int i = 0; i < 16; ++i) {
-                    float y = y16[i] + (bias != nullptr ? __ldg(bias + c0 + i) : 0.f);
-                    if (relu) y = fmaxf(y, 0.f);
-                    y16[i] = y;
-                }
-                if (ystage_lg >= 0) {
-                    char* srow = ystage + ((size_t)row_l << (ystage_lg + 4));
-#pragma unroll
-                    for (int i = 0; i < 4; ++i)
-                        *reinterpret_cast<float4*>(srow + ((((c0 >> 2) + i) ^ (row_l & ncm)) << 4)) =
-                            make_float4(y16[4 * i], y16[4 * i + 1], y16[4 * i + 2], y16[4 * i + 3]);
-                } else {
-                    float* dst = Y + (size_t)row * ldy + c0;
-#pragma unroll
-                    for (int i = 0; i < 16; i += 4) *reinterpret_cast<float4*>(dst + i) = make_float4(y16[i], y16[i + 1], y16[i + 2], y16[i + 3]);
-                }
-            }
-        }
-        if (ystage_lg >= 0) {
-            __syncthreads();                                  // (the epilogue is called by all threads, uniformly)
-            if (!(ko & 2)) {
-                const int m0 = tile * TC_M;
-                for (int e = tid; e < (TC_M << ystage_lg); e += TP_THREADS) {
-                    const int r = e >> ystage_lg, c = e & ncm;
-                    if (m0 + r < M)
-                        *reinterpret_cast<float4*>(Y + (size_t)(m0 + r) * ldy + c * 4) =
-                            *reinterpret_cast<const float4*>(ystage + ((size_t)r << (ystage_lg + 4)) + ((c ^ (r & ncm)) << 4));
-                }
-            }
-        }
-    };
-
-    int it = 0, prev_tile = -1;
-    for (int tile = blockIdx.x; tile < ntiles; tile += gridDim.x, ++it) {
-        const int stage = it % NST;
-        char* Ah = A_hi + (DB ? (size_t)(it & 1) * ab_bytes : 0);
-        char* Al = Ah + KS * a_slab;
-        asm volatile("cp.async.wait_group %0;\n" ::"n"(NST - 1) : "memory");       // this thread's copies of tile `it` landed
-        // single buffer: the MMAs of tile it-1 must have read hi/lo before the split overwrites them.  Double buffer: buffer
-        // it&1 was last read by the MMAs of tile it-2, whose completion every thread observed before its epilogue ran
-        if (!DB && it > 0) tc_mbar_wait(&mma_bar[(it - 1) & 1], (uint32_t)(((it - 1) >> 1) & 1));
-        __syncthreads();                                                            // everyone's copies landed
-        if (!(ko & 4)) {
-            const char* raw = ring + (size_t)stage * stage_bytes;
-#pragma unroll
-            for (int i = 0; i < CPT; ++i) {
-                const int e = i * TP_THREADS + tid;
-                const int r = e / (K / 4), c = e % (K / 4);
-                float4 v = *reinterpret_cast<const float4*>(raw + (size_t)e * 16);
-                if (MASK) {
-                    const float4 mk = *reinterpret_cast<const float4*>(raw + raw_tile + (size_t)e * 16);
-                    v.x = mk.x > 0.f ? v.x : 0.f;
-                    v.y = mk.y > 0.f ? v.y : 0.f;
-                    v.z = mk.z > 0.f ? v.z : 0.f;
-                    v.w = mk.w > 0.f ? v.w : 0.f;
-                }
-                const int s_ = c / 8;
-                tc_store_split(Ah + s_ * a_slab, Al + s_ * a_slab, r, c % 8, v);
-            }
-        }
-        asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-        asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
+        asm volatile("fence.proxy.async.shared::cta;" ::: "memory");      // generic-proxy stores -> async proxy (wgmma)
         __syncthreads();
-        if (tid == 0) {
-            asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-            const uint32_t acc_base = tmem + (uint32_t)((it & 1) * acc_cols);
-            uint32_t acc = 0;
-#pragma unroll 1
-            for (int prod = 0; prod < ((ko & 1) ? 0 : nprod); ++prod) {
-                const char* Ab = (prod < 2) ? Ah : Al;
-                const char* Bb = (prod & 1) ? B_lo : B_hi;
-                for (int s_ = 0; s_ < KS; ++s_) {
+        wg_fence();
 #pragma unroll
-                    for (int k = 0; k < 4; ++k) {
-                        const uint64_t ad = tc_desc(tc_smem_u32(Ab + s_ * a_slab) + k * 32);
-                        const uint64_t bd = tc_desc(tc_smem_u32(Bb + s_ * b_slab) + k * 32);
-                        tc_mma_tf32(acc_base, ad, bd, idesc, acc);
-                        acc = 1;
-                    }
-                }
+        for (int prod = 0; prod < 3; ++prod) {                  // hi*hi, hi*lo, lo*hi
+            const char* Ab = (prod < 2) ? A_hi : A_lo;
+            const char* Bb = (prod & 1) ? B_lo : B_hi;
+#pragma unroll
+            for (int s = 0; s < KS; ++s) {
+#pragma unroll
+                for (int k = 0; k < 4; ++k)                     // 4 MMAs of K = 8 floats (32 bytes) per slab
+                    wgmma_tf32<NW>(acc, wg_desc(wg_smem_u32(Ab + s * a_slab) + k * 32),
+                                   wg_desc(wg_smem_u32(Bb + s * b_slab) + k * 32), (prod | s | k) != 0);
             }
-            tc_commit(&mma_bar[it & 1]);
         }
-        {   // the raw stage just consumed takes tile it + NST
-            const int nt = tile + NST * (int)gridDim.x;
-            if (nt < ntiles) issue_tile(nt, stage);
-            asm volatile("cp.async.commit_group;\n" ::: "memory");
+        wg_commit();
+        if (tile + (int)gridDim.x < ntiles) issue_loads(tile + (int)gridDim.x);
+        wg_wait_all();
+        wg_fence_regs(acc);
+        // epilogue straight from the fragment: each quad of lanes writes 8 consecutive floats (one 32-byte sector) of a row
+        const int r0 = m0 + warp * 16 + (lane >> 2);
+#pragma unroll
+        for (int j = 0; j < NW / 8; ++j) {
+            const int col = 8 * j + 2 * (lane & 3);
+            if (col >= N) continue;
+            const float b0 = bias != nullptr ? __ldg(bias + col) : 0.f;
+            const float b1 = bias != nullptr ? __ldg(bias + col + 1) : 0.f;
+#pragma unroll
+            for (int h = 0; h < 2; ++h) {
+                const int row = r0 + 8 * h;
+                if (row >= M) continue;
+                float y0 = acc[4 * j + 2 * h] + b0, y1 = acc[4 * j + 2 * h + 1] + b1;
+                if (relu) { y0 = fmaxf(y0, 0.f); y1 = fmaxf(y1, 0.f); }
+                *reinterpret_cast<float2*>(Y + (size_t)row * ldy + col) = make_float2(y0, y1);
+            }
         }
-        if (it > 0) {
-            if (DB) tc_mbar_wait(&mma_bar[(it - 1) & 1], (uint32_t)(((it - 1) >> 1) & 1));   // MMAs of tile it-1 (ran under this split)
-            asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-            epilogue(prev_tile, tmem + (uint32_t)(((it - 1) & 1) * acc_cols));
-        }
-        prev_tile = tile;
     }
-    if (it > 0) {
-        tc_mbar_wait(&mma_bar[(it - 1) & 1], (uint32_t)(((it - 1) >> 1) & 1));
-        asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-        epilogue(prev_tile, tmem + (uint32_t)(((it - 1) & 1) * acc_cols));
-    }
-    asm volatile("cp.async.wait_group 0;\n" ::: "memory");
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-    __syncthreads();
-    if (warp == 0) {
-        asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem), "r"(2 * acc_cols) : "memory");
-    }
+}
+
+template <int KS, int NW>
+static int launch_linear_tc(const float* X, int ldx, const float* x_mask, const float* W, const float* bias, float* Y,
+                            int ldy, int M, int N, int relu, cudaStream_t s) {
+    const size_t smem = (size_t)2 * KS * TC_M * 128 + (size_t)2 * KS * NW * 128 + 1024;
+    static_assert((size_t)2 * KS * TC_M * 128 + (size_t)2 * KS * NW * 128 + 1024 <= 227 * 1024, "shared memory");
+    B2R_CUDA_OK(cudaFuncSetAttribute(k_linear_tc<KS, NW>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    int per_sm = 0;
+    B2R_CUDA_OK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_linear_tc<KS, NW>, TC_THREADS, smem));
+    const int ntiles = (M + TC_M - 1) / TC_M;
+    int grid = sm_count() * (per_sm < 1 ? 1 : per_sm);
+    if (grid > ntiles) grid = ntiles;
+    k_linear_tc<KS, NW><<<grid, TC_THREADS, smem, s>>>(X, ldx, x_mask, W, bias, Y, ldy, M, N, relu);
+    B2R_LAUNCH_OK("k_linear_tc");
+    return 0;
+}
+
+template <int KS>
+static int launch_linear_tc_ks(const float* X, int ldx, const float* x_mask, const float* W, const float* bias, float* Y,
+                               int ldy, int M, int N, int relu, cudaStream_t s) {
+    if (N <= 16) return launch_linear_tc<KS, 16>(X, ldx, x_mask, W, bias, Y, ldy, M, N, relu, s);
+    if (N <= 32) return launch_linear_tc<KS, 32>(X, ldx, x_mask, W, bias, Y, ldy, M, N, relu, s);
+    if (N <= 64) return launch_linear_tc<KS, 64>(X, ldx, x_mask, W, bias, Y, ldy, M, N, relu, s);
+    if (N <= 128) return launch_linear_tc<KS, 128>(X, ldx, x_mask, W, bias, Y, ldy, M, N, relu, s);
+    if constexpr (KS <= 2) return launch_linear_tc<KS, 256>(X, ldx, x_mask, W, bias, Y, ldy, M, N, relu, s);
+    // W's hi/lo tiles alone would take 2 * K * 256 * 4 bytes of shared memory
+    return set_error(B2R_E_UNSUPPORTED, "b2r_linear_tc: N=%d with K=%d exceeds the shared memory of one CTA", N, KS * 32);
 }
 
 }  // namespace b2r
@@ -454,71 +178,15 @@ extern "C" int b2r_linear_tc(const float* X, int ldx, const float* x_mask, const
                              int ldy, int64_t M, int N, int K, int relu, b2r_stream_t stream) {
     B2R_REQUIRE(X && W && Y, B2R_E_BADARG, "b2r_linear_fwd_tc: null pointer");
     if (!(K % 32 == 0 && K >= 32 && K <= 128 && N % 16 == 0 && N >= 16 && N <= 256 && M > 0 && M <= 0x7fffffff &&
-          ldx % 4 == 0 && ldy % 4 == 0 && aligned16(X) && aligned16(W) && aligned16(Y)))
+          ldx % 4 == 0 && ldy % 4 == 0 && aligned16(X) && aligned16(W) && aligned16(Y) &&
+          (x_mask == nullptr || aligned16(x_mask))))
         return set_error(B2R_E_UNSUPPORTED, "b2r_linear_fwd_tc: shape M=%lld N=%d K=%d ldx=%d ldy=%d outside the kernel's class",
                          (long long)M, N, K, ldx, ldy);
-    const int KS = K / 32;
-    int cols = 32;
-    while (cols < N) cols <<= 1;
-    static const bool use_pipe = !(getenv("B2R_TC_PIPE") && atoi(getenv("B2R_TC_PIPE")) == 0);
-    static const int nprod = (getenv("B2R_TC_PRODS") && atoi(getenv("B2R_TC_PRODS")) == 4) ? 4 : 3;
-    if (use_pipe && KS <= 2) {
-        // B2R_TC_DB=1: double operand buffers (measured: no gain -- the tile time is set by the epilogue stores and the per-tile
-        // synchronisation, not by split + MMA); B2R_TC_STG=0: direct (row-strided) epilogue stores
-        static const bool want_db = getenv("B2R_TC_DB") && atoi(getenv("B2R_TC_DB")) == 1;
-        static const bool want_stg = !(getenv("B2R_TC_STG") && atoi(getenv("B2R_TC_STG")) == 0);
-        static const int ko = getenv("B2R_TC_KO") ? atoi(getenv("B2R_TC_KO")) : 0;     // diagnostic: wrong results by design
-        const size_t raw_tile = (size_t)TC_M * K * 4;
-        const size_t ab = (size_t)2 * KS * TC_M * 128, wb = (size_t)2 * KS * N * 128;
-        const size_t lim = 227 * 1024 - 64;
-        const size_t smem_db = 2 * ab + wb + 2 * raw_tile + 1024;
-        const bool db = want_db && !x_mask && smem_db <= lim;
-        const int nst = (x_mask || db) ? 2 : 3;
-        size_t psmem = db ? smem_db : ab + wb + nst * raw_tile * (x_mask ? 2 : 1) + 1024;
-        int ystage_lg = -1;
-        if (want_stg && (N == 16 || N == 32 || N == 64 || N == 128) && ldy % 4 == 0 &&
-            psmem + (size_t)TC_M * N * 4 <= lim) {
-            ystage_lg = N == 16 ? 2 : N == 32 ? 3 : N == 64 ? 4 : 5;
-            psmem += (size_t)TC_M * N * 4;
-        }
-        if (psmem <= lim && 2 * cols <= 512) {
-            const int ntiles = (int)((M + TC_M - 1) / TC_M);
-            int grid = sm_count();
-            if (grid > ntiles) grid = ntiles;
-#define B2R_TP(KSV, MK, DBV)                                                                                  \
-    do {                                                                                                      \
-        B2R_CUDA_OK(cudaFuncSetAttribute(k_linear_tc_pipe<KSV, MK, DBV>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)psmem)); \
-        k_linear_tc_pipe<KSV, MK, DBV><<<grid, TP_THREADS, psmem, as_stream(stream)>>>(X, ldx, x_mask, W, bias, Y, ldy, (int)M, N, \
-                                                                                      relu, cols, nprod, ko, ystage_lg); \
-    } while (0)
-            if (KS == 1) { if (x_mask) B2R_TP(1, true, false); else if (db) B2R_TP(1, false, true); else B2R_TP(1, false, false); }
-            else         { if (x_mask) B2R_TP(2, true, false); else if (db) B2R_TP(2, false, true); else B2R_TP(2, false, false); }
-#undef B2R_TP
-            B2R_LAUNCH_OK("k_linear_tc_pipe");
-            return 0;
-        }
+    cudaStream_t s = as_stream(stream);
+    switch (K / 32) {
+        case 1: return launch_linear_tc_ks<1>(X, ldx, x_mask, W, bias, Y, ldy, (int)M, N, relu, s);
+        case 2: return launch_linear_tc_ks<2>(X, ldx, x_mask, W, bias, Y, ldy, (int)M, N, relu, s);
+        case 3: return launch_linear_tc_ks<3>(X, ldx, x_mask, W, bias, Y, ldy, (int)M, N, relu, s);
+        default: return launch_linear_tc_ks<4>(X, ldx, x_mask, W, bias, Y, ldy, (int)M, N, relu, s);
     }
-    const size_t smem = (size_t)2 * KS * TC_M * 128 + (size_t)2 * KS * N * 128 + 1024;
-    if (smem > 200 * 1024) return set_error(B2R_E_UNSUPPORTED, "b2r_linear_fwd_tc: %zu B of shared memory needed", smem);
-    const int ntiles = (int)((M + TC_M - 1) / TC_M);
-    // CTAs per SM: by shared memory (227 KB) and TMEM columns (512), at most 4; B2R_TC_CTAS overrides for A/B
-    int per_sm = (int)((227 * 1024) / (smem + 1024));
-    if (per_sm > 512 / cols) per_sm = 512 / cols;
-    if (per_sm > 4) per_sm = 4;
-    if (per_sm < 1) per_sm = 1;
-    static const int env_ctas = getenv("B2R_TC_CTAS") ? atoi(getenv("B2R_TC_CTAS")) : 0;
-    if (env_ctas > 0 && env_ctas < per_sm) per_sm = env_ctas;
-    // (nprod above: 3 products hi*hi + hi*lo + lo*hi, |err| <= 2^-21 of the fp32 dot, unless B2R_TC_PRODS=4 adds lo*lo)
-    int grid = sm_count() * per_sm;
-    if (grid > ntiles) grid = ntiles;
-#define B2R_TC(KSV)                                                                                    \
-    do {                                                                                               \
-        B2R_CUDA_OK(cudaFuncSetAttribute(k_linear_fwd_tc<KSV>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)); \
-        k_linear_fwd_tc<KSV><<<grid, TC_THREADS, smem, as_stream(stream)>>>(X, ldx, x_mask, W, bias, Y, ldy, (int)M, N, relu, \
-                                                                            cols, nprod);              \
-    } while (0)
-    if (KS == 1) B2R_TC(1); else if (KS == 2) B2R_TC(2); else if (KS == 3) B2R_TC(3); else B2R_TC(4);
-#undef B2R_TC
-    B2R_LAUNCH_OK("k_linear_fwd_tc");
-    return 0;
 }

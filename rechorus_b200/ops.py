@@ -807,7 +807,7 @@ def linear_fwd(x: torch.Tensor, W: torch.Tensor, bias: Optional[torch.Tensor], r
 
 
 def linear_fwd_tc(x: torch.Tensor, W: torch.Tensor, bias: Optional[torch.Tensor], relu: bool, strict: bool = True):
-    """same as linear_fwd on the tcgen05 tensor cores (TF32 hi/lo split, fp32-class accuracy); for shapes outside the
+    """same as linear_fwd on the tensor cores (wgmma, TF32 hi/lo split, fp32-class accuracy); for shapes outside the
     kernel's class it raises (strict) or returns None"""
     _need_cuda(x, W)
     M, ldx = _rows_ld(x)
@@ -838,7 +838,7 @@ def linear_bwd(dy: torch.Tensor, x: torch.Tensor, W: torch.Tensor, y_relu: Optio
         dx = torch.empty((M, K), dtype=torch.float32, device=dy.device)
         done = False
         if _TC_LINEAR and M >= 4096 and N % 32 == 0 and N <= 128 and K % 16 == 0 and K <= 256 and lddy % 4 == 0:
-            # dX = (dY o mask) W = (dY o mask) (W^T)^T on the tcgen05 kernel: the transposed weight (N*K floats) is a copy
+            # dX = (dY o mask) W = (dY o mask) (W^T)^T on the tensor-core kernel: the transposed weight (N*K floats) is a copy
             Wt = W.t().contiguous()
             rc = L.b2r_linear_tc(_p(dy), lddy, _p(y_relu), _p(Wt), None, _p(dx), K, M, K, N, 0, _stream())
             done = rc == 0
@@ -851,7 +851,7 @@ def linear_bwd(dy: torch.Tensor, x: torch.Tensor, W: torch.Tensor, y_relu: Optio
         dW = torch.empty((N, K), dtype=torch.float32, device=dy.device)
         db = torch.empty((N,), dtype=torch.float32, device=dy.device) if need_db else None
         if _TC_DW and M >= 4096 and N % 4 == 0 and N <= 128 and K % 16 == 0 and K <= 240 and lddy % 4 == 0 and ldx % 4 == 0:
-            # long reductions (M = B*L rows) on the tcgen05 tensor cores: k_linear_dw_tc
+            # long reductions (M = B*L rows) on the tensor cores: k_linear_dw_tc
             ws = _ws(L.b2r_linear_bwd_weight_tc_workspace_bytes(M, N, K), dy.device)
             rc = L.b2r_linear_bwd_weight_tc(_p(dy), lddy, _p(y_relu), _p(x), ldx, _p(dW), _p(db), M, N, K, _p(ws), ws.numel(),
                                             _stream())
@@ -866,9 +866,8 @@ def linear_bwd(dy: torch.Tensor, x: torch.Tensor, W: torch.Tensor, y_relu: Optio
     return dx, dW, db
 
 
-# Linear forward and dX with a long batch dimension (M >= 4096) run on the tcgen05 kernels (csrc/linear_tc.cu: TF32 hi/lo
-# split, 3 products, fp32-class accuracy checked in tests/test_gpu_tc.py; the pipelined K <= 64 kernel is ~2x the SGEMM at
-# M = 204800, N = K = 64); B2R_TC_LINEAR=0: CUDA-core SGEMM everywhere
+# Linear forward and dX with a long batch dimension (M >= 4096) run on the tensor cores (csrc/linear_tc.cu: wgmma, TF32
+# hi/lo split, 3 products, fp32-class accuracy checked in tests/test_gpu_tc.py); B2R_TC_LINEAR=0: CUDA-core SGEMM everywhere
 _TC_LINEAR = os.environ.get("B2R_TC_LINEAR", "1") != "0"
 # weight gradients with a long batch reduction run on the tensor cores (csrc/linear_dw_tc.cu); B2R_TC_DW=0: CUDA cores
 _TC_DW = os.environ.get("B2R_TC_DW", "1") != "0"
@@ -885,7 +884,7 @@ class _Linear(torch.autograd.Function):
             x2 = x2.contiguous()
         N, K = W.shape
         if _TC_LINEAR and x2.shape[0] >= 4096 and K % 32 == 0 and K <= 128 and N % 16 == 0 and N <= 256:
-            y = linear_fwd_tc(x2, W, bias, relu, strict=False)          # tcgen05 TF32-split forward
+            y = linear_fwd_tc(x2, W, bias, relu, strict=False)          # wgmma TF32-split forward
         else:
             y = None
         if y is None:

@@ -1,6 +1,6 @@
 """Run the reference's UNCHANGED ``src/main.py`` with the kernel-backed model classes substituted.
 
-    python -m rechorus_b200.overlay --ref /root/reference/src --model_name BPRMF --emb_size 64 --lr 1e-3 \
+    python -m rechorus_b200.overlay --ref /path/to/ReChorus/src --model_name BPRMF --emb_size 64 --lr 1e-3 \
         --l2 1e-6 --dataset Grocery_and_Gourmet_Food --path /tmp/data/ [--table_mode fused]
 
 What it does (SURVEY.md section 8b1): puts the reference ``src/`` on ``sys.path``, restores the NumPy aliases the
@@ -10,8 +10,7 @@ reference's Dataset, reader, runner, argument plumbing and checkpoint code are t
 ``models.general.BPRMF.BPRMF`` etc. with them, and ``runpy``s ``main.py``.  With ``--fused_step 1`` or
 ``--device_metrics 1`` on the command line it also registers ``helpers.B200Runner`` (a subclass of the reference's own
 BaseRunner) through the same by-name discovery.  Needs a CUDA device for the first forward call; there is no CPU
-fallback.  ``--ref`` defaults to /root/reference/src, or to the copy tools/install_reference.py ships in
-baseline/_ref/src (the GPU box has no /root/reference).
+fallback.  ``--ref`` defaults to the unmodified copy build() stages in oracle/_ref/src (oracle/stage_reference.py).
 """
 from __future__ import annotations
 
@@ -20,8 +19,7 @@ import runpy
 import sys
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
-_SHIPPED = os.path.join(os.path.dirname(_HERE), "baseline", "_ref", "src")      # tools/install_reference.py
-DEFAULT_REF = "/root/reference/src" if os.path.isdir("/root/reference/src") else _SHIPPED
+DEFAULT_REF = os.path.join(os.path.dirname(_HERE), "oracle", "_ref", "src")       # oracle/stage_reference.py
 
 
 def _make_runner_module(ref_runner_cls):

@@ -1,4 +1,4 @@
-"""The reference's model plugin contract, re-hosted on the sm_100a kernels.
+"""The reference's model plugin contract, re-hosted on the sm_90a kernels.
 
 ReChorus discovers a model class by name and drives it through a fixed surface (SURVEY.md section 8b1):
 ``parse_model_args`` / ``__init__(args, corpus)`` / ``forward(feed_dict) -> {'prediction': [B, C]}`` /
@@ -6,7 +6,7 @@ ReChorus discovers a model class by name and drives it through a fixed surface (
 This module provides that surface twice:
 
 * stand-alone classes (``BPRMF``, ``NeuMF``, ``SASRec``) usable without the reference checkout -- this is what
-  the tests, ``bench.py`` and ``rechorus_b200.runner.BaseRunner`` use (the GPU box has no /root/reference);
+  the tests, ``bench.py`` and ``rechorus_b200.runner.BaseRunner`` use (they must not need the reference tree);
 * kernel *mixins* (``BPRMFKernels`` ...) that ``rechorus_b200.overlay`` grafts onto the reference's own
   ``GeneralModel`` / ``SequentialModel`` so the reference's unchanged ``src/main.py`` runs them.
 

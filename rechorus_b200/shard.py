@@ -25,7 +25,7 @@ overflow a destination trips a device-side assert.
 
 The global objective is the mean BPR loss over the W*B samples of the step (each rank's local mean / W).
 
-All arithmetic goes through a *backend*: ``CudaBackend`` (the sm_100a kernels; the product) -- the tests inject a
+All arithmetic goes through a *backend*: ``CudaBackend`` (the sm_90a kernels; the product) -- the tests inject a
 CPU stand-in to exercise the exchange bookkeeping under gloo.
 
 Two forms of the exchange:

@@ -1,4 +1,4 @@
-"""pytest wiring: the `gpu` marker (driver runs `-m "not gpu"` on CPU and `-m gpu` on a B200) and path setup."""
+"""pytest wiring: the `gpu` marker (`-m "not gpu"` runs without a GPU, `-m gpu` on an H100) and path setup."""
 import os
 import sys
 
@@ -12,7 +12,7 @@ GOLDEN_DIR = os.path.join(ROOT, "tests", "golden")
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a real B200 (runs the sm_100a kernels through the C-ABI)")
+    config.addinivalue_line("markers", "gpu: needs a real H100 (runs the sm_90a kernels through the C-ABI)")
 
 
 def pytest_collection_modifyitems(config, items):

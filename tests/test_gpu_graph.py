@@ -131,7 +131,6 @@ def test_runner_graph_step_trains_like_the_eager_loop(model_name, extra):
     # the two loops differ in summation order only (the eager one scores shuffled columns); Adam turns a 1e-10 difference
     # of a gradient entry that is within a few orders of eps into a visible fraction of lr (DESIGN.md section 6), so the
     # bulk is bounded tightly and the ill-conditioned tail by the 12 steps' worth of lr = 1e-3 it can drift at most
-    # (measured on a B200: 3e-4 on the first table)
     for (k, pa), (_, pb) in zip(m0.named_parameters(), m1.named_parameters()):
         d = (pa.detach() - pb.detach()).abs().flatten()
         assert float(d.median()) <= 1e-6 and float(d.max()) <= 2e-2, (k, float(d.median()), float(d.max()))

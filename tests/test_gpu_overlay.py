@@ -1,12 +1,13 @@
-"""The drop-in boundary, end to end on a B200: the reference's UNCHANGED ``src/main.py`` (shipped unmodified in
-baseline/_ref by tools/install_reference.py) drives the kernel-backed BPRMF / NeuMF / SASRec through
-``rechorus_b200.overlay``, and the same command line runs the unmodified reference itself on the box's CPU
-(tools/run_reference.py: NumPy alias shim + runpy, nothing else).  Same csv files, same seeds, ``--num_workers 0``: the
-reader, negative sampling, DataLoader order and candidate permutations are the reference's own code in both runs, so the
-two trainings see identical batches and differ only in who does the arithmetic.
+"""The drop-in boundary, end to end on an H100: the reference's UNCHANGED ``src/main.py`` (the unmodified copy build()
+stages in oracle/_ref/src, oracle/stage_reference.py) drives the kernel-backed BPRMF / NeuMF / SASRec through
+``rechorus_b200.overlay``.  The same command line run by the unmodified reference itself on CPU
+(tools/run_reference.py: NumPy alias shim + runpy, nothing else) is stored in tests/golden/overlay_reference.npz
+(tests/golden/make_overlay_golden.py).  Same csv files, same seeds, ``--num_workers 0``: the reader, negative sampling,
+DataLoader order and candidate permutations are the reference's own code in both runs, so the two trainings see identical
+batches and differ only in who does the arithmetic.
 
-Compared: per-epoch losses (the reference's log lines), the dev/test metric lines, and the saved checkpoints
-(``model.save_model`` files interchange, SURVEY.md A.5).  Skipped only where baseline/_ref is absent."""
+Compared: per-epoch losses (the reference's log lines), the Test metric line, and the saved checkpoints
+(``model.save_model`` files interchange, SURVEY.md A.5).  Skipped only where build() had no reference to stage."""
 import os
 import re
 import subprocess
@@ -18,12 +19,12 @@ import pytest
 import torch
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-REF = "/root/reference/src" if os.path.isdir("/root/reference/src") else os.path.join(ROOT, "baseline", "_ref", "src")
+REF = os.path.join(ROOT, "oracle", "_ref", "src")          # oracle/stage_reference.py
+GOLDEN = os.path.join(ROOT, "tests", "golden", "overlay_reference.npz")
 
 pytestmark = [pytest.mark.gpu,
               pytest.mark.skipif(not os.path.isfile(os.path.join(REF, "main.py")),
-                                 reason="unmodified reference not shipped (run tools/install_reference.py where "
-                                        "/root/reference exists)")]
+                                 reason="no unmodified reference staged in oracle/_ref (build() without the checkout)")]
 
 N_USERS, N_ITEMS, ROWS, N_EVAL, N_NEG = 60, 90, 1500, 120, 29
 
@@ -65,6 +66,20 @@ def _run(tmp, tag, launcher, model, extra, gpu):
 
 OVERLAY = ["-m", "rechorus_b200.overlay"]
 REFERENCE = [os.path.join(ROOT, "tools", "run_reference.py")]
+# the reference's CPU runs stored in GOLDEN: tag -> (model, flags)
+REFERENCE_RUNS = {"bprmf_ref": ("BPRMF", ["--num_neg", "3"]),
+                  "sgd_ref": ("BPRMF", ["--num_neg", "7", "--optimizer", "SGD", "--lr", "0.5"]),
+                  "NeuMF_ref": ("NeuMF", ["--num_neg", "2", "--layers", "[32, 16]"]),
+                  "SASRec_ref": ("SASRec", ["--num_neg", "2", "--num_layers", "2", "--num_heads", "2", "--history_max", "8"])}
+
+
+def _reference(tag):
+    """(losses, metrics, checkpoint) of the reference's own CPU run `tag`, from the golden file"""
+    z = np.load(GOLDEN)
+    losses = [float(x) for x in z[tag + "/losses"]]
+    metrics = {k[len(tag) + 8:]: float(z[k]) for k in z.files if k.startswith(tag + "/metric/")}
+    weights = {k[len(tag) + 3:]: torch.from_numpy(z[k]) for k in z.files if k.startswith(tag + "/w/")}
+    return losses, metrics, weights, ""
 
 
 @pytest.fixture(scope="module")
@@ -76,7 +91,7 @@ def workdir(tmp_path_factory):
 
 def test_bprmf_dense_adam_through_unchanged_main_equals_reference_cpu_run(workdir):
     """exact reference semantics: dense gradients into the torch.optim.Adam the reference's runner builds"""
-    l_ref, m_ref, w_ref, _ = _run(workdir, "bprmf_ref", REFERENCE, "BPRMF", ["--num_neg", "3"], "")
+    l_ref, m_ref, w_ref, _ = _reference("bprmf_ref")
     l_gpu, m_gpu, w_gpu, out = _run(workdir, "bprmf_gpu", OVERLAY, "BPRMF", ["--num_neg", "3", "--table_mode", "dense"], "0")
     assert "Device: cuda" in out
     assert len(l_ref) == 2 and np.allclose(l_gpu, l_ref, rtol=0, atol=1e-4), (l_gpu, l_ref)      # logged with 4 decimals
@@ -92,7 +107,7 @@ def test_bprmf_fused_whole_step_route_through_unchanged_main_equals_reference_sg
     unchanged main.py via helpers.B200Runner.  Under SGD without weight decay a row-sparse update IS the dense update,
     so the reference's CPU run is the exact expectation."""
     flags = ["--num_neg", "7", "--optimizer", "SGD", "--lr", "0.5"]
-    l_ref, m_ref, w_ref, _ = _run(workdir, "sgd_ref", REFERENCE, "BPRMF", flags, "")
+    l_ref, m_ref, w_ref, _ = _reference("sgd_ref")
     l_gpu, m_gpu, w_gpu, out = _run(workdir, "sgd_gpu", OVERLAY, "BPRMF",
                                     flags + ["--table_mode", "fused", "--fused_step", "1", "--device_metrics", "1"], "0")
     assert np.allclose(l_gpu, l_ref, rtol=0, atol=1e-4), (l_gpu, l_ref)
@@ -106,7 +121,7 @@ def test_bprmf_fused_whole_step_route_through_unchanged_main_equals_reference_sg
                                          ("SASRec", ["--num_neg", "2", "--num_layers", "2", "--num_heads", "2",
                                                      "--history_max", "8"])])
 def test_deep_models_through_unchanged_main_track_reference_cpu_run(workdir, model, flags):
-    l_ref, m_ref, w_ref, _ = _run(workdir, model + "_ref", REFERENCE, model, flags, "")
+    l_ref, m_ref, w_ref, _ = _reference(model + "_ref")
     l_gpu, m_gpu, w_gpu, _ = _run(workdir, model + "_gpu", OVERLAY, model, flags + ["--table_mode", "dense"], "0")
     assert np.allclose(l_gpu, l_ref, rtol=0, atol=2e-4), (l_gpu, l_ref)
     assert set(w_gpu) == set(w_ref) and all(w_gpu[k].shape == w_ref[k].shape for k in w_ref)

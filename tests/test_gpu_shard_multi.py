@@ -1,4 +1,4 @@
-"""GPU, world_size 2 (needs two B200s on the box; skipped on a single-GPU box): the row-sharded step of config 5 through
+"""GPU, world_size 2 (needs two GPUs on the box; skipped on a single-GPU box): the row-sharded step of config 5 through
 torchrun, both forms of the exchange -- "p2p" (kernels storing into the peers' symmetric-memory buffers, signal-pad
 barriers, no NCCL on the data path) and "nccl" (the collective baseline).  tools/shard_bench.py --check verifies on every
 rank: scores against the all-gathered tables (<= 1e-5) and the SGD step of its shard against the autograd step of the

@@ -1,5 +1,5 @@
-"""GPU: the tcgen05 (TF32 hi/lo split) Linear forward vs fp64, in a subprocess (a descriptor mistake would trap the
-kernel and poison this process's CUDA context)."""
+"""GPU: the wgmma (TF32 hi/lo split) Linear forward and weight gradient vs fp64, each in a subprocess (a descriptor
+mistake would fault the kernel and poison this process's CUDA context)."""
 import os
 import subprocess
 import sys

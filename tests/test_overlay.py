@@ -1,4 +1,4 @@
-"""CPU, build container only: the overlay drives the reference's unchanged main.py up to the first forward,
+"""CPU, on the unmodified reference build() stages in oracle/_ref/src: the overlay drives the reference's unchanged main.py up to the first forward,
 where the kernel-backed class refuses to run without CUDA (no CPU fallback)."""
 import os
 import subprocess
@@ -8,10 +8,10 @@ import numpy as np
 import pandas as pd
 import pytest
 
-REF = "/root/reference/src"
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+REF = os.path.join(ROOT, "oracle", "_ref", "src")          # oracle/stage_reference.py
 
-pytestmark = pytest.mark.skipif(not os.path.isdir(REF), reason="reference checkout not present (GPU box)")
+pytestmark = pytest.mark.skipif(not os.path.isdir(REF), reason="no unmodified reference staged in oracle/_ref (build() without the checkout)")
 
 
 def _tiny_dataset(root):

@@ -1,6 +1,6 @@
-// gather_bench.cu -- stand-alone design-space probe for the K1 gather+dot kernel on B200 (not product code).
-//   nvcc -gencode arch=compute_100a,code=sm_100a -O3 -lineinfo -o build/gather_bench tools/gather_bench.cu
-// Times, with CUDA events after warm-up and with a fresh id set per iteration (table 256 MB > 126 MB L2):
+// gather_bench.cu -- stand-alone design-space probe for the K1 gather+dot kernel (not product code).
+//   nvcc -gencode arch=compute_90a,code=sm_90a -O3 -lineinfo -o build/gather_bench tools/gather_bench.cu
+// Times, with CUDA events after warm-up and with a fresh id set per iteration (table 256 MB > 50 MB L2):
 //   V0  sequential read of the same number of bytes (what "HBM peak" looks like for this byte count)
 //   V1  register-staged LDG.128 gather+dot, RCH rows in flight per lane group, several grid caps
 //   V2  bulk-copy (cp.async.bulk -> shared memory, mbarrier completion) staged gather+dot, 2-stage ring

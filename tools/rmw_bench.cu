@@ -1,5 +1,5 @@
 // rmw_bench.cu -- what HBM can deliver for the access pattern of the row-sparse optimizer (not product code).
-//   nvcc -gencode arch=compute_100a,code=sm_100a -O3 -lineinfo -o build/rmw_bench tools/rmw_bench.cu
+//   nvcc -gencode arch=compute_90a,code=sm_90a -O3 -lineinfo -o build/rmw_bench tools/rmw_bench.cu
 // k_apply_sorted (config 2) touches ~336 k of 1 M rows per step: per row it reads 256 B of weights and 512 B of
 // interleaved Adam state and writes the same 768 B back.  This probe strips everything else away (no pair walk, no
 // contribution gather, trivial arithmetic, registers low enough for full occupancy) and times exactly that traffic,

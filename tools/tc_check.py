@@ -1,6 +1,6 @@
 #!/usr/bin/env python
-"""Check + time b2r_linear_fwd_tc (tcgen05 TF32 hi/lo-split Linear) against fp64 and against the CUDA-core SGEMM.
-Run in its own process (a descriptor mistake traps the kernel and poisons the CUDA context)."""
+"""Check + time b2r_linear_fwd_tc (wgmma TF32 hi/lo-split Linear) against fp64 and against the CUDA-core SGEMM.
+Run in its own process (a descriptor mistake faults the kernel and poisons the CUDA context)."""
 import json
 import os
 import sys
@@ -17,7 +17,7 @@ def main():
     worst = 0.0
     for (M, K, N, relu, bias) in [(128, 64, 64, False, True), (300, 64, 64, True, True), (1000, 32, 16, False, False),
                                   (4096 * 50, 64, 64, False, True), (20480, 128, 64, True, True), (5000, 64, 192, False, True),
-                                  (777, 96, 32, True, True)]:
+                                  (777, 96, 32, True, True), (8192, 64, 256, True, True)]:
         x = (torch.randn(M, K) * 2).cuda()
         W = torch.randn(N, K).cuda()
         b = torch.randn(N).cuda() if bias else None

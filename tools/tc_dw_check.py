@@ -1,6 +1,6 @@
 #!/usr/bin/env python
-"""tcgen05 weight-gradient kernel (csrc/linear_dw_tc.cu) vs fp64 and vs the CUDA-core kernel; timing of both.
-Run in a subprocess by tests/test_gpu_tc.py (a descriptor mistake would trap and poison the CUDA context)."""
+"""wgmma weight-gradient kernel (csrc/linear_dw_tc.cu) vs fp64 and vs the CUDA-core kernel; timing of both.
+Run in a subprocess by tests/test_gpu_tc.py (a descriptor mistake would fault and poison the CUDA context)."""
 import os
 import sys
 
@@ -70,5 +70,6 @@ if __name__ == "__main__":
     run(20481, 16, 32, False, False)         # ragged tail, narrow
     run(20480, 64, 128, False, True, ldpad=64)   # wide input read from a column block of a wider matrix
     run(5000, 128, 64, False, True)
+    run(20480, 64, 192, True, True)          # K > 143: the widest (n = 256) accumulator
     ops.check_ids()
     print("tc dw ok")

@@ -1,7 +1,8 @@
 // tma_gather4_probe.cu -- stand-alone probe (not product code): can the (1+K) x d candidate block of a sample be fetched
 // with TMA tile::gather4 (4 table rows per instruction, one issuing lane, mbarrier completion) faster than per-lane
 // 16-byte cp.async?  Config-2 shape: 4096 samples x 100 random rows of a [1M, 64] fp32 table; gather + dot.
-//   nvcc -gencode arch=compute_100a,code=sm_100a -O3 -lineinfo -o build/tma_gather4_probe tools/tma_gather4_probe.cu -lcuda
+// Blackwell-only: tile::gather4 does not exist on Hopper, so this design probe does not build for sm_90a and nothing
+// in the project builds or runs it (the product kernels use the cp.async path).
 // One warp per sample, 8 warps per CTA: lane 0 arms the warp's mbarrier with 25 x 1024 bytes and issues 25 gather4
 // copies into the warp's 25.6 KB of shared memory; the warp waits and reduces (16 lanes per row).
 #include <cuda.h>
