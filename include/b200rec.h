@@ -281,6 +281,58 @@ B2R_API int b2r_add_layernorm_bwd(const float* dy, const float* x, const float* 
                           int64_t rows, int d, void* ws, size_t ws_bytes, b2r_stream_t stream);
 
 /* ------------------------------------------------------------------------------------------------
+ * Dropout fused into the kernels around it (nn.Dropout of models/general/NeuMF.py:70-72 and the dropout1 / dropout2
+ * of utils/layers.py:113,117).  The mask is a pure function of an element's logical coordinates -- (row r, position t,
+ * column j) of dropout site `site` at training step `step` -- so the backward regenerates it instead of storing it:
+ *   word = Philox4x32-10(counter = (r, (t << 16) | (j >> 2), 0x80000000 | site, lo32(step)),
+ *                        key = (lo32(seed), hi32(seed)))[j & 3];
+ *   kept iff word >= floor(p * 2^32) (nothing at p = 1); kept elements are scaled by float(1 / (1 - p)) (0 at p = 1).
+ * Each element is kept independently with probability 1 - p, as torch's dropout does; torch's own mask bits are not
+ * reproduced.  Bit 31 of counter word 2 separates this stream from b2r_sample_negatives'.
+ * Activation row -> (r, t): L == 0: (row, 0) (NeuMF: r = b*C + c); L > 0 and lengths == NULL: (row / L, row % L)
+ * (SASRec's [B, L, d] block); lengths != NULL: (row, clamp(lengths[row] - 1, 0, L - 1)) (SASRec's last-query block,
+ * one row per sequence at the position select_last reads).  So both SASRec forms draw the same mask, and the mask does
+ * not depend on how far a batch is right-padded beyond its sequences.
+ * ---------------------------------------------------------------------------------------------- */
+typedef struct {
+    const uint64_t* state;     /* DEVICE {seed, step}: the snapshot b2r_dropout_tick wrote for this forward */
+    const int64_t*  lengths;   /* row mapping (see above); NULL unless the rows are one per sequence */
+    double          p;         /* drop probability, 0 <= p <= 1 */
+    int32_t         site;      /* NeuMF: layer index l; SASRec block i: 2i (dropout1), 2i + 1 (dropout2) */
+    int32_t         L;         /* row mapping (see above) */
+} b2r_dropout;
+
+/* snapshot[0..1] = state[0..1] (seed, step), then state[1] += 1.  One thread; enqueued once per training forward, so a
+ * captured CUDA graph advances the step on every replay and a second forward cannot shift the first one's masks. */
+B2R_API int b2r_dropout_tick(uint64_t* state, uint64_t* snapshot, b2r_stream_t stream);
+/* Y = dropout(act(X W^T + bias)): NeuMF.py:70-71 (layer(...).relu() then self.dropout_layer) in one kernel; CUDA-core
+ * (b2r_linear_fwd) and tensor-core (b2r_linear_fwd_tc, same shape class and B2R_E_UNSUPPORTED outside it) forms.  The
+ * backward needs no mask: the saved Y is > 0 exactly where the ReLU passed and the element was kept, so
+ * b2r_linear_bwd_input / b2r_linear_tc with relu_out = Y and the weight scaled by 1 / (1 - p) give dX. */
+B2R_API int b2r_linear_fwd_dropout(const float* X, int ldx, const float* W, const float* bias, float* Y, int ldy,
+                                   int64_t M, int N, int K, int relu, const b2r_dropout* drop, b2r_stream_t stream);
+B2R_API int b2r_linear_fwd_tc_dropout(const float* X, int ldx, const float* W, const float* bias, float* Y, int ldy,
+                                      int64_t M, int N, int K, int relu, const b2r_dropout* drop, b2r_stream_t stream);
+/* b2r_linear_bwd_weight / b2r_linear_bwd_weight_tc of a layer followed by dropout: dW and dbias scaled by 1 / (1 - p)
+ * in the final fixed-order reduction (the autograd of NeuMF.py:71's dropout, helpers/BaseRunner.py:205) */
+B2R_API int b2r_linear_bwd_weight_dropout(const float* dY, int lddy, const float* relu_out, const float* X, int ldx,
+                                          float* dW, float* dbias, int64_t M, int N, int K, const b2r_dropout* drop,
+                                          void* ws, size_t ws_bytes, b2r_stream_t stream);
+B2R_API int b2r_linear_bwd_weight_tc_dropout(const float* dY, int lddy, const float* relu_out, const float* X, int ldx,
+                                             float* dW, float* dbias, int64_t M, int N, int K, const b2r_dropout* drop,
+                                             void* ws, size_t ws_bytes, b2r_stream_t stream);
+/* y = LayerNorm(dropout(x) + res) * gamma + beta: utils/layers.py:113 (layer_norm1(dropout1(context) + seq)) and :117
+ * (layer_norm2(dropout2(output) + context)).  The backward regenerates the mask and writes dres = dz and
+ * dx = dz * mask / (1 - p); workspace as b2r_add_layernorm_bwd.  d <= 256 in both directions. */
+B2R_API int b2r_add_layernorm_fwd_dropout(const float* x, const float* res, const float* gamma, const float* beta, float* y,
+                                          float* mean, float* rstd, int64_t rows, int d, float eps, const b2r_dropout* drop,
+                                          b2r_stream_t stream);
+B2R_API int b2r_add_layernorm_bwd_dropout(const float* dy, const float* x, const float* res, const float* gamma,
+                                          const float* mean, const float* rstd, float* dz, float* dx, float* dgamma,
+                                          float* dbeta, int64_t rows, int d, const b2r_dropout* drop, void* ws,
+                                          size_t ws_bytes, b2r_stream_t stream);
+
+/* ------------------------------------------------------------------------------------------------
  * SASRec sequence kernels (models/sequential/SASRec.py:51-86, utils/layers.py:34-63).
  *   embed_history : x[b,t,:] = I[hist[b,t]] + P[(len[b]-t) * (hist[b,t] > 0)]; pos_out (optional) gets the
  *                   position index used per element                                    (SASRec.py:58-66)

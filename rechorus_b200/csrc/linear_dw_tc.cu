@@ -14,6 +14,7 @@
 // a second kernel adds the CTAs' partials in CTA order (fixed order -> deterministic).
 #include "common.cuh"
 #include "wgmma_tf32.cuh"
+#include "dropout.cuh"
 
 namespace b2r {
 
@@ -146,9 +147,12 @@ k_linear_dw_tc(const float* __restrict__ dY, int lddy, const float* __restrict__
     }
 }
 
-// dW[n, k] = sum_c part[c][n][k], dbias[n] = sum_c part[c][n][K]  (c ascending)
+// dW[n, k] = sum_c part[c][n][k], dbias[n] = sum_c part[c][n][K]  (c ascending); SCALED: times `scale` (the 1 / (1 - p)
+// of a dropout after the layer)
+template <bool SCALED = false>
 __global__ void __launch_bounds__(256)
-k_linear_dw_reduce(const float* __restrict__ part, int ctas, int N, int K, float* __restrict__ dW, float* __restrict__ dbias) {
+k_linear_dw_reduce(const float* __restrict__ part, int ctas, int N, int K, float* __restrict__ dW, float* __restrict__ dbias,
+                   float scale) {
     // 8 lanes per output element: lane l adds CTAs l, l+8, ... (ascending), then a fixed shuffle tree -> deterministic
     const int total = N * (K + 1);
     const int cl = threadIdx.x & 7;
@@ -160,6 +164,7 @@ k_linear_dw_reduce(const float* __restrict__ part, int ctas, int N, int K, float
         a += __shfl_xor_sync(B2R_FULL_MASK, a, 1);
         a += __shfl_xor_sync(B2R_FULL_MASK, a, 2);
         a += __shfl_xor_sync(B2R_FULL_MASK, a, 4);
+        if constexpr (SCALED) a *= scale;
         if (cl == 0 && i < total) {
             const int n = i / (K + 1), k = i % (K + 1);
             if (k < K) dW[(size_t)n * K + k] = a;
@@ -170,7 +175,7 @@ k_linear_dw_reduce(const float* __restrict__ part, int ctas, int N, int K, float
 
 template <int NB>
 static int launch_linear_dw_tc(const float* dY, int lddy, const float* relu_out, const float* X, int ldx, float* dW,
-                               float* dbias, int M, int N, int K, float* part, cudaStream_t s) {
+                               float* dbias, int M, int N, int K, float* part, const float* scale, cudaStream_t s) {
     const int nwg = (N + 63) / 64;
     const size_t smem = (size_t)2 * DW_SLABS * nwg * 64 * 128 + (size_t)2 * DW_SLABS * NB * 128 + 1024;
     B2R_CUDA_OK(cudaFuncSetAttribute(k_linear_dw_tc<NB>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
@@ -185,9 +190,28 @@ static int launch_linear_dw_tc(const float* dY, int lddy, const float* relu_out,
     k_linear_dw_tc<NB><<<ctas, 128 * nwg, smem, s>>>(dY, lddy, relu_out, X, ldx, part, M, N, K, rows_per_cta);
     B2R_LAUNCH_OK("k_linear_dw_tc");
     const int total = N * (K + 1);
-    k_linear_dw_reduce<<<(total + 31) / 32, 256, 0, s>>>(part, ctas, N, K, dW, dbias);
+    if (scale != nullptr) k_linear_dw_reduce<true><<<(total + 31) / 32, 256, 0, s>>>(part, ctas, N, K, dW, dbias, *scale);
+    else k_linear_dw_reduce<<<(total + 31) / 32, 256, 0, s>>>(part, ctas, N, K, dW, dbias, 1.f);
     B2R_LAUNCH_OK("k_linear_dw_reduce");
     return 0;
+}
+
+static int linear_bwd_weight_tc(const float* dY, int lddy, const float* relu_out, const float* X, int ldx, float* dW,
+                                float* dbias, int64_t M, int N, int K, void* ws, size_t ws_bytes, const float* scale,
+                                cudaStream_t s) {
+    B2R_REQUIRE(dY && X && dW && ws, B2R_E_BADARG, "b2r_linear_bwd_weight_tc: null pointer");
+    if (!(N % 4 == 0 && N >= 4 && N <= 64 * DW_MAX_WG && K % 16 == 0 && K >= 16 && K <= 240 && M > 0 &&
+          M <= 0x7fffffff && lddy % 4 == 0 && ldx % 4 == 0 && lddy >= N && ldx >= K && aligned16(dY) && aligned16(X) &&
+          (relu_out == nullptr || aligned16(relu_out))))
+        return set_error(B2R_E_UNSUPPORTED, "b2r_linear_bwd_weight_tc: shape M=%lld N=%d K=%d outside the kernel's class",
+                         (long long)M, N, K);
+    B2R_REQUIRE(ws_bytes >= b2r_linear_bwd_weight_tc_workspace_bytes(M, N, K), B2R_E_WORKSPACE,
+                "b2r_linear_bwd_weight_tc: workspace too small");
+    float* part = static_cast<float*>(ws);
+    // wgmma width: K features + the ones row, rounded up to the instantiated widths
+    if (K + 1 <= 48) return launch_linear_dw_tc<48>(dY, lddy, relu_out, X, ldx, dW, dbias, (int)M, N, K, part, scale, s);
+    if (K + 1 <= 80) return launch_linear_dw_tc<80>(dY, lddy, relu_out, X, ldx, dW, dbias, (int)M, N, K, part, scale, s);
+    return launch_linear_dw_tc<256>(dY, lddy, relu_out, X, ldx, dW, dbias, (int)M, N, K, part, scale, s);
 }
 
 }  // namespace b2r
@@ -204,18 +228,14 @@ extern "C" size_t b2r_linear_bwd_weight_tc_workspace_bytes(int64_t M, int N, int
 extern "C" int b2r_linear_bwd_weight_tc(const float* dY, int lddy, const float* relu_out, const float* X, int ldx, float* dW,
                                         float* dbias, int64_t M, int N, int K, void* ws, size_t ws_bytes,
                                         b2r_stream_t stream) {
-    B2R_REQUIRE(dY && X && dW && ws, B2R_E_BADARG, "b2r_linear_bwd_weight_tc: null pointer");
-    if (!(N % 4 == 0 && N >= 4 && N <= 64 * DW_MAX_WG && K % 16 == 0 && K >= 16 && K <= 240 && M > 0 &&
-          M <= 0x7fffffff && lddy % 4 == 0 && ldx % 4 == 0 && lddy >= N && ldx >= K && aligned16(dY) && aligned16(X) &&
-          (relu_out == nullptr || aligned16(relu_out))))
-        return set_error(B2R_E_UNSUPPORTED, "b2r_linear_bwd_weight_tc: shape M=%lld N=%d K=%d outside the kernel's class",
-                         (long long)M, N, K);
-    B2R_REQUIRE(ws_bytes >= b2r_linear_bwd_weight_tc_workspace_bytes(M, N, K), B2R_E_WORKSPACE,
-                "b2r_linear_bwd_weight_tc: workspace too small");
-    cudaStream_t s = as_stream(stream);
-    float* part = static_cast<float*>(ws);
-    // wgmma width: K features + the ones row, rounded up to the instantiated widths
-    if (K + 1 <= 48) return launch_linear_dw_tc<48>(dY, lddy, relu_out, X, ldx, dW, dbias, (int)M, N, K, part, s);
-    if (K + 1 <= 80) return launch_linear_dw_tc<80>(dY, lddy, relu_out, X, ldx, dW, dbias, (int)M, N, K, part, s);
-    return launch_linear_dw_tc<256>(dY, lddy, relu_out, X, ldx, dW, dbias, (int)M, N, K, part, s);
+    return linear_bwd_weight_tc(dY, lddy, relu_out, X, ldx, dW, dbias, M, N, K, ws, ws_bytes, nullptr, as_stream(stream));
+}
+
+extern "C" int b2r_linear_bwd_weight_tc_dropout(const float* dY, int lddy, const float* relu_out, const float* X, int ldx,
+                                                float* dW, float* dbias, int64_t M, int N, int K, const b2r_dropout* drop,
+                                                void* ws, size_t ws_bytes, b2r_stream_t stream) {
+    const int rc = check_dropout(drop, "b2r_linear_bwd_weight_tc_dropout");
+    if (rc != 0) return rc;
+    const float scale = dropout_scale(drop->p);
+    return linear_bwd_weight_tc(dY, lddy, relu_out, X, ldx, dW, dbias, M, N, K, ws, ws_bytes, &scale, as_stream(stream));
 }

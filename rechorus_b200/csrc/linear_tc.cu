@@ -15,6 +15,7 @@
 // flight through the MMAs and the epilogue, which adds the bias, applies ReLU and stores Y straight from the accumulator.
 #include "common.cuh"
 #include "wgmma_tf32.cuh"
+#include "dropout.cuh"
 
 namespace b2r {
 
@@ -37,11 +38,12 @@ __device__ __forceinline__ void tc_store_split(char* hi_base, char* lo_base, int
 }
 
 // dynamic shared memory (1024-byte aligned): A_hi[KS][64*128B] A_lo[...] B_hi[KS][NW*128B] B_lo[...]; NW >= N is the
-// wgmma width, W's rows N..NW-1 are zero and their output columns are not stored
-template <int KS, int NW>
+// wgmma width, W's rows N..NW-1 are zero and their output columns are not stored.  DROP: dropout (dropout.cuh) after
+// bias / ReLU in the epilogue, output row = activation row
+template <int KS, int NW, bool DROP = false>
 __global__ void __launch_bounds__(TC_THREADS)
 k_linear_tc(const float* __restrict__ X, int ldx, const float* __restrict__ amask, const float* __restrict__ W,
-            const float* __restrict__ bias, float* __restrict__ Y, int ldy, int M, int N, int relu) {
+            const float* __restrict__ bias, float* __restrict__ Y, int ldy, int M, int N, int relu, DropK dk) {
     extern __shared__ __align__(1024) unsigned char smem_raw[];
     constexpr int K = KS * 32;                              // KS 128-byte K slabs
     constexpr int LPT = 8 * KS * TC_M / TC_THREADS;         // 16-byte loads per thread per tile
@@ -86,6 +88,8 @@ k_linear_tc(const float* __restrict__ X, int ldx, const float* __restrict__ amas
     float acc[NW / 2];
 #pragma unroll
     for (int i = 0; i < NW / 2; ++i) acc[i] = 0.f;
+    DropKey key;
+    if constexpr (DROP) key = drop_key(dk);
     int tile = blockIdx.x;
     if (tile < ntiles) issue_loads(tile);
     for (; tile < ntiles; tile += gridDim.x) {
@@ -124,44 +128,76 @@ k_linear_tc(const float* __restrict__ X, int ldx, const float* __restrict__ amas
             if (col >= N) continue;
             const float b0 = bias != nullptr ? __ldg(bias + col) : 0.f;
             const float b1 = bias != nullptr ? __ldg(bias + col + 1) : 0.f;
+            uint2 wd[2];                                        // DROP: mask words of (col, col + 1) in rows r0, r0 + 8
+            if constexpr (DROP) {
+                // lanes l and l ^ 1 hold the four columns of one group in the same two rows: the even lane draws row r0's
+                // words, the odd lane row r0 + 8's, and each hands its partner the half the partner needs
+                const int odd = lane & 1;
+                const uint4 w = drop_words(dk, key, min(r0 + 8 * odd, M - 1), (uint32_t)col >> 2);
+                const uint32_t g0 = __shfl_xor_sync(B2R_FULL_MASK, odd ? w.x : w.z, 1);
+                const uint32_t g1 = __shfl_xor_sync(B2R_FULL_MASK, odd ? w.y : w.w, 1);
+                wd[0] = odd ? make_uint2(g0, g1) : make_uint2(w.x, w.y);
+                wd[1] = odd ? make_uint2(w.z, w.w) : make_uint2(g0, g1);
+            }
 #pragma unroll
             for (int h = 0; h < 2; ++h) {
                 const int row = r0 + 8 * h;
                 if (row >= M) continue;
                 float y0 = acc[4 * j + 2 * h] + b0, y1 = acc[4 * j + 2 * h + 1] + b1;
                 if (relu) { y0 = fmaxf(y0, 0.f); y1 = fmaxf(y1, 0.f); }
+                if constexpr (DROP) {
+                    y0 = drop_apply(dk, wd[h].x, y0);
+                    y1 = drop_apply(dk, wd[h].y, y1);
+                }
                 *reinterpret_cast<float2*>(Y + (size_t)row * ldy + col) = make_float2(y0, y1);
             }
         }
     }
 }
 
-template <int KS, int NW>
+template <int KS, int NW, bool DROP>
 static int launch_linear_tc(const float* X, int ldx, const float* x_mask, const float* W, const float* bias, float* Y,
-                            int ldy, int M, int N, int relu, cudaStream_t s) {
+                            int ldy, int M, int N, int relu, const DropK& dk, cudaStream_t s) {
     const size_t smem = (size_t)2 * KS * TC_M * 128 + (size_t)2 * KS * NW * 128 + 1024;
     static_assert((size_t)2 * KS * TC_M * 128 + (size_t)2 * KS * NW * 128 + 1024 <= 227 * 1024, "shared memory");
-    B2R_CUDA_OK(cudaFuncSetAttribute(k_linear_tc<KS, NW>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    B2R_CUDA_OK(cudaFuncSetAttribute(k_linear_tc<KS, NW, DROP>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     int per_sm = 0;
-    B2R_CUDA_OK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_linear_tc<KS, NW>, TC_THREADS, smem));
+    B2R_CUDA_OK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_linear_tc<KS, NW, DROP>, TC_THREADS, smem));
     const int ntiles = (M + TC_M - 1) / TC_M;
     int grid = sm_count() * (per_sm < 1 ? 1 : per_sm);
     if (grid > ntiles) grid = ntiles;
-    k_linear_tc<KS, NW><<<grid, TC_THREADS, smem, s>>>(X, ldx, x_mask, W, bias, Y, ldy, M, N, relu);
+    k_linear_tc<KS, NW, DROP><<<grid, TC_THREADS, smem, s>>>(X, ldx, x_mask, W, bias, Y, ldy, M, N, relu, dk);
     B2R_LAUNCH_OK("k_linear_tc");
     return 0;
 }
 
-template <int KS>
+template <int KS, bool DROP>
 static int launch_linear_tc_ks(const float* X, int ldx, const float* x_mask, const float* W, const float* bias, float* Y,
-                               int ldy, int M, int N, int relu, cudaStream_t s) {
-    if (N <= 16) return launch_linear_tc<KS, 16>(X, ldx, x_mask, W, bias, Y, ldy, M, N, relu, s);
-    if (N <= 32) return launch_linear_tc<KS, 32>(X, ldx, x_mask, W, bias, Y, ldy, M, N, relu, s);
-    if (N <= 64) return launch_linear_tc<KS, 64>(X, ldx, x_mask, W, bias, Y, ldy, M, N, relu, s);
-    if (N <= 128) return launch_linear_tc<KS, 128>(X, ldx, x_mask, W, bias, Y, ldy, M, N, relu, s);
-    if constexpr (KS <= 2) return launch_linear_tc<KS, 256>(X, ldx, x_mask, W, bias, Y, ldy, M, N, relu, s);
+                               int ldy, int M, int N, int relu, const DropK& dk, cudaStream_t s) {
+    if (N <= 16) return launch_linear_tc<KS, 16, DROP>(X, ldx, x_mask, W, bias, Y, ldy, M, N, relu, dk, s);
+    if (N <= 32) return launch_linear_tc<KS, 32, DROP>(X, ldx, x_mask, W, bias, Y, ldy, M, N, relu, dk, s);
+    if (N <= 64) return launch_linear_tc<KS, 64, DROP>(X, ldx, x_mask, W, bias, Y, ldy, M, N, relu, dk, s);
+    if (N <= 128) return launch_linear_tc<KS, 128, DROP>(X, ldx, x_mask, W, bias, Y, ldy, M, N, relu, dk, s);
+    if constexpr (KS <= 2) return launch_linear_tc<KS, 256, DROP>(X, ldx, x_mask, W, bias, Y, ldy, M, N, relu, dk, s);
     // W's hi/lo tiles alone would take 2 * K * 256 * 4 bytes of shared memory
     return set_error(B2R_E_UNSUPPORTED, "b2r_linear_tc: N=%d with K=%d exceeds the shared memory of one CTA", N, KS * 32);
+}
+
+template <bool DROP>
+static int linear_tc(const float* X, int ldx, const float* x_mask, const float* W, const float* bias, float* Y, int ldy,
+                     int64_t M, int N, int K, int relu, const DropK& dk, cudaStream_t s) {
+    B2R_REQUIRE(X && W && Y, B2R_E_BADARG, "b2r_linear_fwd_tc: null pointer");
+    if (!(K % 32 == 0 && K >= 32 && K <= 128 && N % 16 == 0 && N >= 16 && N <= 256 && M > 0 && M <= 0x7fffffff &&
+          ldx % 4 == 0 && ldy % 4 == 0 && aligned16(X) && aligned16(W) && aligned16(Y) &&
+          (x_mask == nullptr || aligned16(x_mask))))
+        return set_error(B2R_E_UNSUPPORTED, "b2r_linear_fwd_tc: shape M=%lld N=%d K=%d ldx=%d ldy=%d outside the kernel's class",
+                         (long long)M, N, K, ldx, ldy);
+    switch (K / 32) {
+        case 1: return launch_linear_tc_ks<1, DROP>(X, ldx, x_mask, W, bias, Y, ldy, (int)M, N, relu, dk, s);
+        case 2: return launch_linear_tc_ks<2, DROP>(X, ldx, x_mask, W, bias, Y, ldy, (int)M, N, relu, dk, s);
+        case 3: return launch_linear_tc_ks<3, DROP>(X, ldx, x_mask, W, bias, Y, ldy, (int)M, N, relu, dk, s);
+        default: return launch_linear_tc_ks<4, DROP>(X, ldx, x_mask, W, bias, Y, ldy, (int)M, N, relu, dk, s);
+    }
 }
 
 }  // namespace b2r
@@ -176,17 +212,12 @@ extern "C" int b2r_linear_fwd_tc(const float* X, int ldx, const float* W, const 
 
 extern "C" int b2r_linear_tc(const float* X, int ldx, const float* x_mask, const float* W, const float* bias, float* Y,
                              int ldy, int64_t M, int N, int K, int relu, b2r_stream_t stream) {
-    B2R_REQUIRE(X && W && Y, B2R_E_BADARG, "b2r_linear_fwd_tc: null pointer");
-    if (!(K % 32 == 0 && K >= 32 && K <= 128 && N % 16 == 0 && N >= 16 && N <= 256 && M > 0 && M <= 0x7fffffff &&
-          ldx % 4 == 0 && ldy % 4 == 0 && aligned16(X) && aligned16(W) && aligned16(Y) &&
-          (x_mask == nullptr || aligned16(x_mask))))
-        return set_error(B2R_E_UNSUPPORTED, "b2r_linear_fwd_tc: shape M=%lld N=%d K=%d ldx=%d ldy=%d outside the kernel's class",
-                         (long long)M, N, K, ldx, ldy);
-    cudaStream_t s = as_stream(stream);
-    switch (K / 32) {
-        case 1: return launch_linear_tc_ks<1>(X, ldx, x_mask, W, bias, Y, ldy, (int)M, N, relu, s);
-        case 2: return launch_linear_tc_ks<2>(X, ldx, x_mask, W, bias, Y, ldy, (int)M, N, relu, s);
-        case 3: return launch_linear_tc_ks<3>(X, ldx, x_mask, W, bias, Y, ldy, (int)M, N, relu, s);
-        default: return launch_linear_tc_ks<4>(X, ldx, x_mask, W, bias, Y, ldy, (int)M, N, relu, s);
-    }
+    return linear_tc<false>(X, ldx, x_mask, W, bias, Y, ldy, M, N, K, relu, DropK{}, as_stream(stream));
+}
+
+extern "C" int b2r_linear_fwd_tc_dropout(const float* X, int ldx, const float* W, const float* bias, float* Y, int ldy,
+                                         int64_t M, int N, int K, int relu, const b2r_dropout* drop, b2r_stream_t stream) {
+    const int rc = check_dropout(drop, "b2r_linear_fwd_tc_dropout");
+    if (rc != 0) return rc;
+    return linear_tc<true>(X, ldx, nullptr, W, bias, Y, ldy, M, N, K, relu, make_dropk(*drop), as_stream(stream));
 }

@@ -12,26 +12,9 @@
 // Philox4x32-10(counter = (lo32(i*K+j), hi32(i*K+j), 0, epoch), key = seed).  The same definition is restated in
 // oracle.device_sampler_reference, so the GPU output is checked bit for bit.
 #include "common.cuh"
+#include "philox.cuh"
 
 namespace b2r {
-
-__device__ __forceinline__ uint32_t philox4x32_10_word0(uint32_t c0, uint32_t c1, uint32_t c2, uint32_t c3,
-                                                        uint32_t k0, uint32_t k1) {
-    constexpr uint32_t M0 = 0xD2511F53u, M1 = 0xCD9E8D57u, W0 = 0x9E3779B9u, W1 = 0xBB67AE85u;
-#pragma unroll
-    for (int r = 0; r < 10; ++r) {
-        const uint32_t hi0 = __umulhi(M0, c0), lo0 = M0 * c0;
-        const uint32_t hi1 = __umulhi(M1, c2), lo1 = M1 * c2;
-        const uint32_t n0 = hi1 ^ c1 ^ k0, n2 = hi0 ^ c3 ^ k1;
-        c0 = n0;
-        c1 = lo1;
-        c2 = n2;
-        c3 = lo0;
-        k0 += W0;
-        k1 += W1;
-    }
-    return c0;
-}
 
 __global__ void __launch_bounds__(256)
 k_sample_negatives(const int64_t* __restrict__ user_ids, int64_t N, int K, const int64_t* __restrict__ clicked_ptr,
@@ -53,7 +36,7 @@ k_sample_negatives(const int64_t* __restrict__ user_ids, int64_t N, int K, const
             out[idx] = 1;
             continue;
         }
-        const uint32_t x = philox4x32_10_word0((uint32_t)idx, (uint32_t)((uint64_t)idx >> 32), 0u, epoch, seed_lo, seed_hi);
+        const uint32_t x = philox4x32_10((uint32_t)idx, (uint32_t)((uint64_t)idx >> 32), 0u, epoch, seed_lo, seed_hi).x;
         const int64_t r = (int64_t)(((uint64_t)x * (uint64_t)A) >> 32);
         int64_t lo = 0, hi = m;                            // p = first position with c[p] - 1 - p > r
         while (lo < hi) {

@@ -35,6 +35,12 @@ class BprmfTables(C.Structure):
                 ("d", C.c_int32), ("_pad", C.c_int32)]
 
 
+class Dropout(C.Structure):
+    """b2r_dropout (include/b200rec.h)"""
+    _fields_ = [("state", C.c_void_p), ("lengths", C.c_void_p), ("p", C.c_double), ("site", C.c_int32),
+                ("L", C.c_int32)]
+
+
 OPT_SGD, OPT_ADAM, OPT_ADAGRAD = 0, 1, 2
 PROF_SCORE_FWD, PROF_SCORE_BWDQ, PROF_SEGMENT_I, PROF_SEGMENT_U, PROF_PLAN_I, PROF_LOSS = range(6)
 
@@ -105,6 +111,21 @@ SIGNATURES = {
     "b2r_add_layernorm_fwd": (C.c_int, [C.c_void_p] * 7 + [C.c_int64, C.c_int, C.c_float, C.c_void_p]),
     "b2r_add_layernorm_bwd_workspace_bytes": (C.c_size_t, [C.c_int64, C.c_int]),
     "b2r_add_layernorm_bwd": (C.c_int, [C.c_void_p] * 9 + [C.c_int64, C.c_int, C.c_void_p, C.c_size_t, C.c_void_p]),
+    "b2r_dropout_tick": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p]),
+    "b2r_linear_fwd_dropout": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int64,
+                                         C.c_int, C.c_int, C.c_int, C.POINTER(Dropout), C.c_void_p]),
+    "b2r_linear_fwd_tc_dropout": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int64,
+                                            C.c_int, C.c_int, C.c_int, C.POINTER(Dropout), C.c_void_p]),
+    "b2r_linear_bwd_weight_dropout": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p,
+                                                C.c_void_p, C.c_int64, C.c_int, C.c_int, C.POINTER(Dropout), C.c_void_p,
+                                                C.c_size_t, C.c_void_p]),
+    "b2r_linear_bwd_weight_tc_dropout": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p,
+                                                   C.c_void_p, C.c_int64, C.c_int, C.c_int, C.POINTER(Dropout), C.c_void_p,
+                                                   C.c_size_t, C.c_void_p]),
+    "b2r_add_layernorm_fwd_dropout": (C.c_int, [C.c_void_p] * 7 + [C.c_int64, C.c_int, C.c_float, C.POINTER(Dropout),
+                                                                   C.c_void_p]),
+    "b2r_add_layernorm_bwd_dropout": (C.c_int, [C.c_void_p] * 10 + [C.c_int64, C.c_int, C.POINTER(Dropout), C.c_void_p,
+                                                                    C.c_size_t, C.c_void_p]),
     "b2r_embed_history": (C.c_int, [C.c_void_p, C.c_int64, C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p,
                                     C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p]),
     "b2r_attention_fwd": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.c_int,

@@ -822,9 +822,90 @@ def linear_fwd_tc(x: torch.Tensor, W: torch.Tensor, bias: Optional[torch.Tensor]
     return y
 
 
+# --------------------------------------------------------------------------------------------------
+# dropout (NeuMF.py:70-72, utils/layers.py:113-117) fused into the Linear and residual-LayerNorm kernels
+# --------------------------------------------------------------------------------------------------
+
+class DropoutState:
+    """One model's dropout stream on the device: int64 {seed, step} (b2r_dropout in include/b200rec.h).  ``tick()``
+    enqueues b2r_dropout_tick, which copies {seed, step} into a fresh 16-byte snapshot and advances step; every kernel of
+    that forward and of its backward reads the snapshot.  Captured in a CUDA graph, the tick advances on every replay."""
+
+    def __init__(self, seed: int, device):
+        self.state = torch.tensor([_i64(seed), 0], dtype=torch.int64, device=device)
+
+    def tick(self) -> torch.Tensor:
+        snap = torch.empty(2, dtype=torch.int64, device=self.state.device)
+        _lib.check(_lib.load().b2r_dropout_tick(_p(self.state), _p(snap), _stream()), "b2r_dropout_tick")
+        return snap
+
+    def get(self) -> Tuple[int, int]:
+        """(seed, step) -- the step the next training forward uses (synchronises)"""
+        seed, step = (int(v) for v in self.state.cpu())
+        return seed & 0xFFFFFFFFFFFFFFFF, step
+
+    def set(self, seed: int, step: int) -> None:
+        self.state.copy_(torch.tensor([_i64(seed), int(step)], dtype=torch.int64))
+
+
+def _i64(v: int) -> int:
+    v = int(v) & 0xFFFFFFFFFFFFFFFF
+    return v - (1 << 64) if v >= (1 << 63) else v
+
+
+def check_dropout_p(p: float) -> float:
+    """nn.Dropout's validation (the reference builds nn.Dropout(p): ValueError outside [0, 1])"""
+    if not 0.0 <= float(p) <= 1.0:
+        raise ValueError(f"dropout probability has to be between 0 and 1, but got {p}")
+    return float(p)
+
+
+@dataclass
+class Drop:
+    """One dropout site of one forward: the snapshot DropoutState.tick() returned, the probability and the site index
+    (NeuMF layer l: l; SASRec block i: 2i after the attention, 2i + 1 after linear2)."""
+    snapshot: torch.Tensor
+    p: float
+    site: int
+
+    def c_struct(self, L: int = 0, lengths: Optional[torch.Tensor] = None) -> _lib.Dropout:
+        return _lib.Dropout(_p(self.snapshot), _p(lengths), float(self.p), int(self.site), int(L))
+
+    @property
+    def scale(self) -> float:
+        """s = float(1 / (1 - p)), 0 at p = 1"""
+        import numpy as np
+        return 0.0 if self.p >= 1.0 else float(np.float32(1.0 / (1.0 - self.p)))
+
+
+def linear_fwd_dropout(x: torch.Tensor, W: torch.Tensor, bias: Optional[torch.Tensor], relu: bool, drop: Drop,
+                       tc: bool) -> torch.Tensor:
+    """y = dropout(act(x W^T + b)) in one kernel, rows = activation rows (NeuMF's r = b*C + c); tc: the tensor-core kernel
+    where the shape is in its class, else the CUDA-core one"""
+    _need_cuda(x, W, drop.snapshot)
+    M, ldx = _rows_ld(x)
+    N, K = W.shape
+    W = _f32c(W, "W")
+    y = torch.empty((M, N), dtype=torch.float32, device=x.device)
+    L = _lib.load()
+    dc = drop.c_struct()
+    rc = -3
+    if tc:
+        rc = L.b2r_linear_fwd_tc_dropout(_p(x), ldx, _p(W), _p(bias), _p(y), N, M, N, K, 1 if relu else 0, C.byref(dc),
+                                         _stream())
+        if rc not in (0, -3):
+            _lib.check(rc, "b2r_linear_fwd_tc_dropout")
+    if rc != 0:
+        _lib.check(L.b2r_linear_fwd_dropout(_p(x), ldx, _p(W), _p(bias), _p(y), N, M, N, K, 1 if relu else 0, C.byref(dc),
+                                            _stream()), "b2r_linear_fwd_dropout")
+    return y
+
+
 def linear_bwd(dy: torch.Tensor, x: torch.Tensor, W: torch.Tensor, y_relu: Optional[torch.Tensor],
-               need_dx: bool, need_dw: bool, need_db: bool):
-    """gradients of y = act(x W^T + b) given dy; y_relu = saved post-ReLU output (None when no ReLU)."""
+               need_dx: bool, need_dw: bool, need_db: bool, drop: Optional[Drop] = None):
+    """gradients of y = act(x W^T + b) given dy; y_relu = saved post-ReLU output (None when no ReLU).  drop: the layer's
+    output went through that dropout (y_relu is then the saved post-dropout output, > 0 exactly where ReLU and mask
+    passed): dz = s * dy * [y > 0], with s folded into the weight for dX and into the final reduction for dW / dbias."""
     M, lddy = _rows_ld(dy)
     _, ldx = _rows_ld(x)
     N, K = W.shape
@@ -837,15 +918,16 @@ def linear_bwd(dy: torch.Tensor, x: torch.Tensor, W: torch.Tensor, y_relu: Optio
     if need_dx:
         dx = torch.empty((M, K), dtype=torch.float32, device=dy.device)
         done = False
+        Wd = W if drop is None else W * drop.scale
         if _TC_LINEAR and M >= 4096 and N % 32 == 0 and N <= 128 and K % 16 == 0 and K <= 256 and lddy % 4 == 0:
             # dX = (dY o mask) W = (dY o mask) (W^T)^T on the tensor-core kernel: the transposed weight (N*K floats) is a copy
-            Wt = W.t().contiguous()
+            Wt = Wd.t().contiguous()
             rc = L.b2r_linear_tc(_p(dy), lddy, _p(y_relu), _p(Wt), None, _p(dx), K, M, K, N, 0, _stream())
             done = rc == 0
             if rc not in (0, -3):
                 _lib.check(rc, "b2r_linear_tc")
         if not done:
-            _lib.check(L.b2r_linear_bwd_input(_p(dy), lddy, _p(y_relu), _p(W), _p(dx), K, M, N, K, _stream()),
+            _lib.check(L.b2r_linear_bwd_input(_p(dy), lddy, _p(y_relu), _p(Wd), _p(dx), K, M, N, K, _stream()),
                        "b2r_linear_bwd_input")
     if need_dw or need_db:
         dW = torch.empty((N, K), dtype=torch.float32, device=dy.device)
@@ -853,16 +935,27 @@ def linear_bwd(dy: torch.Tensor, x: torch.Tensor, W: torch.Tensor, y_relu: Optio
         if _TC_DW and M >= 4096 and N % 4 == 0 and N <= 128 and K % 16 == 0 and K <= 240 and lddy % 4 == 0 and ldx % 4 == 0:
             # long reductions (M = B*L rows) on the tensor cores: k_linear_dw_tc
             ws = _ws(L.b2r_linear_bwd_weight_tc_workspace_bytes(M, N, K), dy.device)
-            rc = L.b2r_linear_bwd_weight_tc(_p(dy), lddy, _p(y_relu), _p(x), ldx, _p(dW), _p(db), M, N, K, _p(ws), ws.numel(),
-                                            _stream())
+            if drop is None:
+                rc = L.b2r_linear_bwd_weight_tc(_p(dy), lddy, _p(y_relu), _p(x), ldx, _p(dW), _p(db), M, N, K, _p(ws),
+                                                ws.numel(), _stream())
+            else:
+                dc = drop.c_struct()
+                rc = L.b2r_linear_bwd_weight_tc_dropout(_p(dy), lddy, _p(y_relu), _p(x), ldx, _p(dW), _p(db), M, N, K,
+                                                        C.byref(dc), _p(ws), ws.numel(), _stream())
             if rc == 0:
                 return dx, dW, db
             if rc != -3:                                   # B2R_E_UNSUPPORTED falls through to the CUDA-core kernel
                 _lib.check(rc, "b2r_linear_bwd_weight_tc")
         nbytes = L.b2r_linear_bwd_weight_workspace_bytes(M, N, K)
         ws = _ws(nbytes, dy.device)
-        _lib.check(L.b2r_linear_bwd_weight(_p(dy), lddy, _p(y_relu), _p(x), ldx, _p(dW), _p(db), M, N, K, _p(ws),
-                                           ws.numel(), _stream()), "b2r_linear_bwd_weight")
+        if drop is None:
+            _lib.check(L.b2r_linear_bwd_weight(_p(dy), lddy, _p(y_relu), _p(x), ldx, _p(dW), _p(db), M, N, K, _p(ws),
+                                               ws.numel(), _stream()), "b2r_linear_bwd_weight")
+        else:
+            dc = drop.c_struct()
+            _lib.check(L.b2r_linear_bwd_weight_dropout(_p(dy), lddy, _p(y_relu), _p(x), ldx, _p(dW), _p(db), M, N, K,
+                                                       C.byref(dc), _p(ws), ws.numel(), _stream()),
+                       "b2r_linear_bwd_weight_dropout")
     return dx, dW, db
 
 
@@ -874,23 +967,29 @@ _TC_DW = os.environ.get("B2R_TC_DW", "1") != "0"
 
 
 class _Linear(torch.autograd.Function):
-    """nn.Linear (+ optional ReLU) on the library's SGEMM: NeuMF.py:70 / layers.py:26-28,106-107."""
+    """nn.Linear (+ optional ReLU, + optional dropout after the ReLU) on the library's SGEMM: NeuMF.py:70-71 /
+    layers.py:26-28,106-107."""
 
     @staticmethod
-    def forward(ctx, x, W, bias, relu):
+    def forward(ctx, x, W, bias, relu, drop=None):
         shape = x.shape
         x2 = x.reshape(-1, shape[-1])
         if x2.stride(1) != 1:
             x2 = x2.contiguous()
         N, K = W.shape
-        if _TC_LINEAR and x2.shape[0] >= 4096 and K % 32 == 0 and K <= 128 and N % 16 == 0 and N <= 256:
+        tc = _TC_LINEAR and x2.shape[0] >= 4096 and K % 32 == 0 and K <= 128 and N % 16 == 0 and N <= 256
+        if drop is not None:
+            if not relu:
+                raise ValueError("fused dropout follows a ReLU (its backward reads the mask off the saved output)")
+            y = linear_fwd_dropout(x2, W, bias, relu, drop, tc)
+        elif tc:
             y = linear_fwd_tc(x2, W, bias, relu, strict=False)          # wgmma TF32-split forward
         else:
             y = None
         if y is None:
             y = linear_fwd(x2, W, bias, relu)
         ctx.save_for_backward(x2, W, y if relu else None)
-        ctx.has_bias, ctx.shape = bias is not None, shape
+        ctx.has_bias, ctx.shape, ctx.drop = bias is not None, shape, drop
         return y.view(*shape[:-1], W.shape[0])
 
     @staticmethod
@@ -898,21 +997,22 @@ class _Linear(torch.autograd.Function):
         x2, W, y_relu = ctx.saved_tensors
         dy2 = _f32c(dy.reshape(-1, W.shape[0]), "dy")
         dx, dW, db = linear_bwd(dy2, x2, W, y_relu, ctx.needs_input_grad[0], ctx.needs_input_grad[1],
-                                ctx.has_bias and ctx.needs_input_grad[2])
+                                ctx.has_bias and ctx.needs_input_grad[2], ctx.drop)
         if dx is not None:
             dx = dx.view(*ctx.shape)
-        return dx, dW, db, None
+        return dx, dW, db, None, None
 
 
-def linear(x, W, bias=None, relu=False):
-    return _Linear.apply(x, W, bias, relu)
+def linear(x, W, bias=None, relu=False, drop: Optional[Drop] = None):
+    """drop: dropout after the ReLU (NeuMF.py:71), fused into the kernel; needs relu=True"""
+    return _Linear.apply(x, W, bias, relu, drop)
 
 
 class _AddLayerNorm(torch.autograd.Function):
-    """LayerNorm(x + res) with affine (layers.py:113,117)."""
+    """LayerNorm(x + res) with affine (layers.py:113,117); with ``drop``, LayerNorm(dropout(x) + res)."""
 
     @staticmethod
-    def forward(ctx, x, res, gamma, beta, eps):
+    def forward(ctx, x, res, gamma, beta, eps, drop=None, lengths=None, L_seq=0):
         _need_cuda(x, res, gamma, beta)
         d = x.shape[-1]
         x2, r2 = _f32c(x.reshape(-1, d), "x"), _f32c(res.reshape(-1, d), "res")
@@ -921,15 +1021,21 @@ class _AddLayerNorm(torch.autograd.Function):
         mean = torch.empty(rows, dtype=torch.float32, device=x.device)
         rstd = torch.empty(rows, dtype=torch.float32, device=x.device)
         L = _lib.load()
-        _lib.check(L.b2r_add_layernorm_fwd(_p(x2), _p(r2), _p(gamma), _p(beta), _p(y), _p(mean), _p(rstd), rows, d,
-                                           float(eps), _stream()), "b2r_add_layernorm_fwd")
-        ctx.save_for_backward(x2, r2, gamma, mean, rstd)
-        ctx.shape = x.shape
+        if drop is None:
+            _lib.check(L.b2r_add_layernorm_fwd(_p(x2), _p(r2), _p(gamma), _p(beta), _p(y), _p(mean), _p(rstd), rows, d,
+                                               float(eps), _stream()), "b2r_add_layernorm_fwd")
+        else:
+            _need_cuda(drop.snapshot, lengths)
+            dc = drop.c_struct(L_seq, lengths)
+            _lib.check(L.b2r_add_layernorm_fwd_dropout(_p(x2), _p(r2), _p(gamma), _p(beta), _p(y), _p(mean), _p(rstd), rows,
+                                                       d, float(eps), C.byref(dc), _stream()), "b2r_add_layernorm_fwd_dropout")
+        ctx.save_for_backward(x2, r2, gamma, mean, rstd, lengths)
+        ctx.shape, ctx.drop, ctx.L_seq = x.shape, drop, L_seq
         return y.view(x.shape)
 
     @staticmethod
     def backward(ctx, dy):
-        x2, r2, gamma, mean, rstd = ctx.saved_tensors
+        x2, r2, gamma, mean, rstd, lengths = ctx.saved_tensors
         d = x2.shape[1]
         rows = x2.shape[0]
         dy2 = _f32c(dy.reshape(-1, d), "dy")
@@ -938,14 +1044,31 @@ class _AddLayerNorm(torch.autograd.Function):
         db = torch.empty(d, dtype=torch.float32, device=dy.device)
         L = _lib.load()
         ws = _ws(L.b2r_add_layernorm_bwd_workspace_bytes(rows, d), dy.device)
-        _lib.check(L.b2r_add_layernorm_bwd(_p(dy2), _p(x2), _p(r2), _p(gamma), _p(mean), _p(rstd), _p(dz), _p(dg),
-                                           _p(db), rows, d, _p(ws), ws.numel(), _stream()), "b2r_add_layernorm_bwd")
-        dz = dz.view(ctx.shape)
-        return dz, dz, dg, db, None
+        if ctx.drop is None:
+            _lib.check(L.b2r_add_layernorm_bwd(_p(dy2), _p(x2), _p(r2), _p(gamma), _p(mean), _p(rstd), _p(dz), _p(dg),
+                                               _p(db), rows, d, _p(ws), ws.numel(), _stream()), "b2r_add_layernorm_bwd")
+            dz = dz.view(ctx.shape)
+            return dz, dz, dg, db, None, None, None, None
+        dx = torch.empty_like(x2)
+        dc = ctx.drop.c_struct(ctx.L_seq, lengths)
+        _lib.check(L.b2r_add_layernorm_bwd_dropout(_p(dy2), _p(x2), _p(r2), _p(gamma), _p(mean), _p(rstd), _p(dz), _p(dx),
+                                                   _p(dg), _p(db), rows, d, C.byref(dc), _p(ws), ws.numel(), _stream()),
+                   "b2r_add_layernorm_bwd_dropout")
+        return dx.view(ctx.shape), dz.view(ctx.shape), dg, db, None, None, None, None
 
 
-def add_layernorm(x, res, gamma, beta, eps=1e-5):
-    return _AddLayerNorm.apply(x, res, gamma, beta, eps)
+def add_layernorm(x, res, gamma, beta, eps=1e-5, drop: Optional[Drop] = None, lengths: Optional[torch.Tensor] = None,
+                  seq_len: int = 0):
+    """drop: LayerNorm(dropout(x) + res) (layers.py:113,117).  Rows map to (sequence, position) for the mask: x [B, L, d]
+    gives row b*L + t -> (b, t); x [B, d] with ``lengths`` and ``seq_len`` (the batch's padded width) gives row b ->
+    (b, clamp(lengths[b] - 1, 0, seq_len - 1)), the position select_last reads"""
+    if drop is not None and lengths is None:
+        if x.dim() != 3:
+            raise ValueError("add_layernorm with dropout: x must be [B, L, d], or [B, d] with lengths")
+        seq_len = x.shape[1]
+    elif lengths is not None:
+        lengths = _i64c(lengths, "lengths")
+    return _AddLayerNorm.apply(x, res, gamma, beta, eps, drop, lengths, int(seq_len))
 
 
 # B2R_ATTN=v1: the first (shared-memory operand) attention kernels for every shape, for A/B

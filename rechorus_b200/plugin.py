@@ -89,6 +89,35 @@ class _KernelModelMixin:
             ops.poll_ids(tables[0].device)
         return super().train(mode)
 
+    # Dropout (NeuMF.py:70-72, layers.py:113-117) runs inside the Linear / residual-LayerNorm kernels with a counter-based
+    # mask (include/b200rec.h, b2r_dropout).  Its seed is torch.initial_seed() at construction -- read, not drawn, so the
+    # reference's CPU RNG streams stay in step -- and its step counter lives on the device, ticked once per training
+    # forward (so a captured CUDA graph advances it on every replay).  Neither is part of the state_dict.
+    def _dropout_init(self) -> None:
+        self.__dict__["_b2r_drop_seed"] = torch.initial_seed()
+
+    def _dropout_state(self, device) -> "ops.DropoutState":
+        st = self.__dict__.get("_b2r_drop_state")
+        if st is None:
+            seed = self.__dict__.get("_b2r_drop_seed")
+            st = ops.DropoutState(torch.initial_seed() if seed is None else seed, device)
+            self.__dict__["_b2r_drop_state"] = st
+        return st
+
+    def _dropout_snapshot(self, device):
+        """the forward's {seed, step} snapshot (one tick), or None when no dropout applies (p = 0 or eval mode)"""
+        if not (self.training and self.dropout > 0):
+            return None
+        return self._dropout_state(device).tick()
+
+    def dropout_rng_state(self):
+        """(seed, step) of the dropout stream: the next training forward draws its masks at this step"""
+        dev = next(self.parameters()).device
+        return self._dropout_state(dev).get()
+
+    def set_dropout_rng_state(self, seed: int, step: int) -> None:
+        self._dropout_state(next(self.parameters()).device).set(seed, step)
+
     # models/BaseModel.py:175-189
     def loss(self, out_dict: dict) -> torch.Tensor:
         return ops.bpr_loss(out_dict["prediction"])
@@ -214,6 +243,7 @@ class NeuMFKernels(_KernelModelMixin):
         if self.emb_size % 4 != 0:
             raise ValueError("rechorus_b200 kernels need emb_size % 4 == 0")
         self.layers = list(ast.literal_eval(args.layers))      # the reference eval()s this string (NeuMF.py:38)
+        self._dropout_init()
         self._define_params()
         self.apply(self.init_weights)
         self._register_tables(self.mf_u_embeddings.weight, self.mf_i_embeddings.weight,
@@ -247,10 +277,11 @@ class NeuMFKernels(_KernelModelMixin):
         pred = ops.score(ops.colscale(mf_u, w_out[0, :d]), self.mf_i_embeddings.weight, i_ids)
         # MLP tower on [mlp_u[b] ; mlp_i[id]]
         h = ops.gather_concat(self.mlp_u_embeddings.weight, self.mlp_i_embeddings.weight, u_ids, i_ids)
-        for layer in self.mlp:
-            h = ops.linear(h, layer.weight, layer.bias, relu=True)
-            if self.dropout > 0:
-                h = self.dropout_layer(h)
+        snap = self._dropout_snapshot(u_ids.device)
+        for l, layer in enumerate(self.mlp):
+            # relu, then self.dropout_layer (site l of the mask), in the Linear kernel's epilogue
+            drop = None if snap is None else ops.Drop(snap, self.dropout_layer.p, l)
+            h = ops.linear(h, layer.weight, layer.bias, relu=True, drop=drop)
         pred = pred + ops.linear(h, w_out[:, d:], None, relu=False).view(B, C)
         return {"prediction": pred.view(feed_dict["batch_size"], -1)}
 
@@ -297,6 +328,8 @@ class SASRecKernels(_KernelModelMixin):
         self.num_heads = args.num_heads
         if self.emb_size % 4 != 0 or self.emb_size % self.num_heads != 0:
             raise ValueError("rechorus_b200 kernels need emb_size % 4 == 0 and emb_size % num_heads == 0")
+        ops.check_dropout_p(self.dropout)                     # the reference's nn.Dropout(dropout) (layers.py:104,110)
+        self._dropout_init()
         self._base_define_params()
         self.apply(self.init_weights)
         self._register_tables(self.i_embeddings.weight, mode=getattr(args, "table_mode", "dense"))
@@ -308,10 +341,17 @@ class SASRecKernels(_KernelModelMixin):
         self.transformer_block = nn.ModuleList(
             [_TransformerParams(self.emb_size, self.emb_size) for _ in range(self.num_layers)])
 
-    def _last_block_one_query(self, blk, x, history, lengths):
+    def _drops(self, snap, bi):
+        if snap is None:
+            return None, None
+        return ops.Drop(snap, self.dropout, 2 * bi), ops.Drop(snap, self.dropout, 2 * bi + 1)
+
+    def _last_block_one_query(self, blk, x, history, lengths, snap=None, bi=0):
         """The last block for the only position whose output SASRec uses (len-1, SASRec.py:74-81): keys and values from
         every position, query / residual LayerNorms / FFN for that one row per sequence.  Same result as the full block
-        followed by select_last (dropout-free path only; with dropout the full block runs)."""
+        followed by select_last, dropout included: the masks are keyed by (sequence, position), not by buffer row."""
+        d1, d2 = self._drops(snap, bi)
+        Lb = history.shape[1]
         a = blk.masked_attn_head
         ones = torch.ones_like(history)
         x_last = ops.select_last(x, ones, lengths)                               # raw row len-1 (no padding mask yet)
@@ -319,33 +359,32 @@ class SASRecKernels(_KernelModelMixin):
         k = ops.linear(x, a.k_linear.weight, a.k_linear.bias)
         v = ops.linear(x, a.v_linear.weight, a.v_linear.bias)
         ctx_last = ops.attention_last(q_last, k, v, lengths, self.num_heads)
-        c = ops.add_layernorm(ctx_last, x_last, blk.layer_norm1.weight, blk.layer_norm1.bias)
+        c = ops.add_layernorm(ctx_last, x_last, blk.layer_norm1.weight, blk.layer_norm1.bias, drop=d1, lengths=lengths,
+                              seq_len=Lb)
         o = ops.linear(ops.linear(c, blk.linear1.weight, blk.linear1.bias, relu=True), blk.linear2.weight, blk.linear2.bias)
-        y = ops.add_layernorm(o, c, blk.layer_norm2.weight, blk.layer_norm2.bias)  # [B, d]
+        y = ops.add_layernorm(o, c, blk.layer_norm2.weight, blk.layer_norm2.bias, drop=d2, lengths=lengths,
+                              seq_len=Lb)  # [B, d]
         t_last = (lengths - 1).clamp(0, history.shape[1] - 1)
         valid = (history.gather(1, t_last.view(-1, 1)) > 0).to(y.dtype)            # SASRec.py:74: y * valid_his
         return y * valid
 
-    def user_state(self, history, lengths):
+    def user_state(self, history, lengths, snap=None):
+        """snap: the forward's dropout snapshot (None: no dropout)"""
         x = ops.embed_history(self.i_embeddings.weight, self.p_embeddings.weight, history, lengths)   # [B, L, d]
-        p = self.dropout
         n_blocks = len(self.transformer_block)
         for bi, blk in enumerate(self.transformer_block):
-            if _SASREC_LASTQ and bi == n_blocks - 1 and not (p > 0):
-                return self._last_block_one_query(blk, x, history, lengths)
+            if _SASREC_LASTQ and bi == n_blocks - 1:
+                return self._last_block_one_query(blk, x, history, lengths, snap, bi)
+            d1, d2 = self._drops(snap, bi)
             a = blk.masked_attn_head
             q = ops.linear(x, a.q_linear.weight, a.q_linear.bias)
             k = ops.linear(x, a.k_linear.weight, a.k_linear.bias)
             v = ops.linear(x, a.v_linear.weight, a.v_linear.bias)
             ctx = ops.causal_attention(q, k, v, self.num_heads, live=lengths if _SASREC_LIVE else None)
-            if p > 0:
-                ctx = torch.nn.functional.dropout(ctx, p, self.training)
-            c = ops.add_layernorm(ctx, x, blk.layer_norm1.weight, blk.layer_norm1.bias)
+            c = ops.add_layernorm(ctx, x, blk.layer_norm1.weight, blk.layer_norm1.bias, drop=d1)       # dropout1 fused
             o = ops.linear(ops.linear(c, blk.linear1.weight, blk.linear1.bias, relu=True),
                            blk.linear2.weight, blk.linear2.bias)
-            if p > 0:
-                o = torch.nn.functional.dropout(o, p, self.training)
-            x = ops.add_layernorm(o, c, blk.layer_norm2.weight, blk.layer_norm2.bias)
+            x = ops.add_layernorm(o, c, blk.layer_norm2.weight, blk.layer_norm2.bias, drop=d2)         # dropout2 fused
         return ops.select_last(x, history, lengths)                                                    # [B, d]
 
     def query_rows(self, feed_dict):
@@ -357,7 +396,7 @@ class SASRecKernels(_KernelModelMixin):
         i_ids = feed_dict["item_id"]            # [B, C]
         history = feed_dict["history_items"]    # [B, Lb] right-padded with 0
         lengths = feed_dict["lengths"]          # [B]
-        h = self.user_state(history, lengths)
+        h = self.user_state(history, lengths, self._dropout_snapshot(history.device))
         pred = ops.score(h, self.i_embeddings.weight, i_ids)
         out = {"prediction": pred.view(history.shape[0], -1)}
         if getattr(self, "_b2r_vectors", False):                       # SASRec.py:83-86, kept by SASRecImpression (:121-122)

@@ -226,8 +226,10 @@ class BaseRunner:
         (rechorus_b200.graph.GraphedStep) and replayed for every batch of the captured shape: one launch per step instead of
         ~70 (NeuMF) to ~150 (SASRec).  The first full-size batch trains through the capture's eager warm-up step; the ragged
         last batch runs eagerly.  As in ``_fit_whole_steps`` the per-row candidate permutation of :189 is drawn (RNG stream in
-        step with the reference) but not applied: it is a no-op for candidates scored independently.  Models with dropout keep
-        the eager loop (``fit`` does not route them here)."""
+        step with the reference) but not applied: it is a no-op for candidates scored independently.  With dropout it is
+        still one in distribution: every element's mask is drawn independently (keyed by its position, not by the
+        candidate's identity), so permuting the candidate columns leaves the distribution of the step unchanged.  The
+        dropout step counter lives on the device and advances on every replay."""
         from .graph import GraphedStep
         model = dataset.model
         dl = DataLoader(dataset, batch_size=self.batch_size, shuffle=True, num_workers=self.num_workers,
@@ -341,7 +343,7 @@ class BaseRunner:
         model.train()
         if self.fused_step and hasattr(model, "train_step") and isinstance(model.optimizer, RowSparseOptimizer):
             return self._fit_whole_steps(dataset, epoch)
-        if self.graph_step and isinstance(model.optimizer, RowSparseOptimizer) and not getattr(model, "dropout", 0):
+        if self.graph_step and isinstance(model.optimizer, RowSparseOptimizer):
             return self._fit_graphed(dataset, epoch)
         losses = []
         dl = DataLoader(dataset, batch_size=self.batch_size, shuffle=True, num_workers=self.num_workers,
