@@ -410,6 +410,16 @@ B2R_API int b2r_sample_negatives(const int64_t* user_ids, int64_t N, int K, cons
  * out_uid[t] = users[row], out_iid[t, 0] = items[row], out_iid[t, 1 + k] = neg[row, k]. */
 B2R_API int b2r_collate_general(const int64_t* users, const int64_t* items, const int64_t* neg, const int64_t* perm,
                                 int64_t start, int Bn, int K, int64_t* out_uid, int64_t* out_iid, b2r_stream_t stream);
+/* The history part of a SequentialModel training batch (SequentialModel.Dataset._get_feed_dict, models/BaseModel.py:236-245,
+ * + the padding of collate_batch, :135-152), right-padded to the fixed width Lp: batch row t is training row
+ * perm[start + t] (perm NULL: start + t); with u = users[row], p = positions[row] and len = H > 0 ? min(p, H) : p,
+ * out_hist[t, j] = his_items[his_ptr[u] + p - len + j] for j < len, else 0, and out_len[t] = len.  out_hist int64
+ * [Bn, Lp], out_len int64 [Bn]; his_ptr [n_users+1] / his_items is the CSR of corpus.user_his (items only).  Bad rows
+ * (u out of range, p < 1, p beyond the user's history, len > Lp) are clamped inside the CSR and counted in err_flag. */
+B2R_API int b2r_collate_history(const int64_t* users, const int64_t* positions, const int64_t* his_ptr,
+                                const int64_t* his_items, int64_t n_users, const int64_t* perm, int64_t start, int Bn,
+                                int H, int Lp, int64_t* out_hist, int64_t* out_len, int32_t* err_flag,
+                                b2r_stream_t stream);
 
 /* ------------------------------------------------------------------------------------------------
  * Groundwork for the exact dense-Adam mode (not used by the default paths of this round): advance rows of a table whose

@@ -1,5 +1,6 @@
 // sampler.cu -- SURVEY.md §8 row f3, batch production on the device (opt-in: --device_sampler / --device_batches):
-// the per-epoch negative sampling of models/BaseModel.py:206-214 and the collate of models/BaseModel.py:192-203,135-152.
+// the per-epoch negative sampling of models/BaseModel.py:206-214 and the collate of models/BaseModel.py:192-203,135-152
+// (plus the history slice of :236-245 for sequential models).
 //
 // Reference semantics: for every training row i (user u_i) and every j < K draw an item uniformly from [1, n_items)
 // and redraw while it is in the user's training clicks -- the result is uniform over the user's non-clicked items,
@@ -68,6 +69,38 @@ k_collate_general(const int64_t* __restrict__ users, const int64_t* __restrict__
     }
 }
 
+// The history part of a SequentialModel training batch: what SequentialModel.Dataset._get_feed_dict
+// (models/BaseModel.py:236-245) slices per sample, right-padded with 0 as collate_batch (:135-152) does, but to the fixed
+// width Lp instead of the batch maximum.  Row t is training row perm[start + t] (perm NULL: identity); with u = users[row],
+// p = positions[row] and len = H > 0 ? min(p, H) : p, out_hist[t, j] = his_items[his_ptr[u] + p - len + j] for j < len,
+// else 0; out_len[t] = len.  Bad input (u out of range, p < 1, p beyond the user's history, len > Lp) is clamped to
+// something readable inside the CSR and counted once per row in err_flag.
+__global__ void __launch_bounds__(256)
+k_collate_history(const int64_t* __restrict__ users, const int64_t* __restrict__ positions,
+                  const int64_t* __restrict__ his_ptr, const int64_t* __restrict__ his_items, int64_t n_users,
+                  const int64_t* __restrict__ perm, int64_t start, int Bn, int H, int Lp, int64_t* __restrict__ out_hist,
+                  int64_t* __restrict__ out_len, int32_t* __restrict__ err_flag) {
+    const int64_t total = (int64_t)Bn * Lp;
+    for (int64_t idx = (int64_t)blockIdx.x * 256 + threadIdx.x; idx < total; idx += (int64_t)gridDim.x * 256) {
+        const int t = (int)(idx / Lp), j = (int)(idx - (int64_t)t * Lp);
+        const int64_t row = perm ? perm[start + t] : start + t;
+        int64_t u = users[row], p = positions[row];
+        bool bad = false;
+        if (u < 0 || u >= n_users) { bad = true; u = 0; }
+        const int64_t beg = his_ptr[u];
+        const int64_t m = his_ptr[u + 1] - beg;
+        if (p < 1) { bad = true; p = 0; }
+        if (p > m) { bad = true; p = m; }
+        int64_t len = (H > 0 && p > H) ? H : p;
+        if (len > Lp) { bad = true; len = Lp; }
+        if (j == 0) {
+            out_len[t] = len;
+            if (bad && err_flag) atomicAdd(err_flag, 1);
+        }
+        out_hist[idx] = j < len ? his_items[beg + p - len + j] : 0;
+    }
+}
+
 }  // namespace b2r
 
 using namespace b2r;
@@ -83,6 +116,25 @@ extern "C" int b2r_collate_general(const int64_t* users, const int64_t* items, c
     if (grid > cap) grid = cap;
     k_collate_general<<<(int)grid, 256, 0, as_stream(stream)>>>(users, items, neg, perm, start, Bn, K, out_uid, out_iid);
     B2R_LAUNCH_OK("k_collate_general");
+    return 0;
+}
+
+extern "C" int b2r_collate_history(const int64_t* users, const int64_t* positions, const int64_t* his_ptr,
+                                   const int64_t* his_items, int64_t n_users, const int64_t* perm, int64_t start, int Bn,
+                                   int H, int Lp, int64_t* out_hist, int64_t* out_len, int32_t* err_flag,
+                                   b2r_stream_t stream) {
+    B2R_REQUIRE(users && positions && his_ptr && his_items && out_hist && out_len, B2R_E_BADARG,
+                "b2r_collate_history: null pointer");
+    B2R_REQUIRE(Bn >= 0 && Lp >= 1 && n_users >= 1 && start >= 0, B2R_E_BADARG,
+                "b2r_collate_history: Bn=%d Lp=%d n_users=%lld", Bn, Lp, (long long)n_users);
+    if (Bn == 0) return 0;
+    const int64_t total = (int64_t)Bn * Lp;
+    int64_t grid = (total + 255) / 256;
+    const int64_t cap = (int64_t)sm_count() * 8;
+    if (grid > cap) grid = cap;
+    k_collate_history<<<(int)grid, 256, 0, as_stream(stream)>>>(users, positions, his_ptr, his_items, n_users, perm, start,
+                                                                Bn, H, Lp, out_hist, out_len, err_flag);
+    B2R_LAUNCH_OK("k_collate_history");
     return 0;
 }
 

@@ -6,8 +6,9 @@ pays one launch and the GPU sees them back to back.
 What makes the capture legal: every kernel of this package is enqueued on ``torch.cuda.current_stream()`` without host
 synchronisation, scratch memory comes from torch's caching allocator (graph-private pool during capture), and the
 optimizer's per-step scalars (Adam's bias corrections) live on the device (``RowSparseOptimizer(device_clock=True)``,
-``b2r_optim_tick``) instead of in kernel parameters.  Batches are copied into static device buffers before each replay;
-shapes are fixed at capture time (a ragged last batch goes through the eager path).
+``b2r_optim_tick``) instead of in kernel parameters.  Batches are copied into static device buffers before each replay
+(or, with ``replay()``, written there by the caller's own device collate); shapes are fixed at capture time (a ragged last
+batch goes through the eager path).
 
 One precondition comes from autograd, not from this package: a parameter's AccumulateGrad node is bound to the stream
 that was current when the node was created and lives as long as any autograd graph that reaches it.  If the caller still
@@ -68,5 +69,11 @@ class GraphedStep:
         device scalar: read or clone it before the next replay)"""
         for k, s in self.shapes.items():
             self.static[k].copy_(feed[k], non_blocking=True)
+        self.graph.replay()
+        return self.loss
+
+    def replay(self) -> torch.Tensor:
+        """replay on whatever the static input tensors (``self.static``) hold now, with no copy: for a producer that writes
+        each batch straight into them on the current stream (runner.fit_on_device).  Returns the step's loss, as ``__call__``"""
         self.graph.replay()
         return self.loss

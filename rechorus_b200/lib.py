@@ -159,6 +159,8 @@ SIGNATURES = {
                                        C.c_uint64, C.c_uint32, C.c_void_p, C.c_void_p, C.c_void_p]),
     "b2r_collate_general": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_int, C.c_int,
                                       C.c_void_p, C.c_void_p, C.c_void_p]),
+    "b2r_collate_history": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p, C.c_int64,
+                                      C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
     "b2r_attention_last_fwd": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p,
                                          C.c_int, C.c_int, C.c_int, C.c_int, C.c_void_p]),
     "b2r_attention_last_bwd": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p,

@@ -289,6 +289,82 @@ def collate_general(users: torch.Tensor, items: torch.Tensor, neg: torch.Tensor,
                                                _p(out_uid), _p(out_iid), _stream()), "b2r_collate_general")
 
 
+def history_csr(user_his: dict, n_users: int):
+    """corpus.user_his ({u: [(item, time), ...]}, helpers/SeqReader.py:14-33) as a CSR over users: his_ptr int64
+    [n_users + 1] and his_items int64 [total] (items only), user u's history at his_items[his_ptr[u]:his_ptr[u + 1]].
+    NumPy arrays; one pass over the interactions."""
+    import numpy as np
+    ptr = np.zeros(int(n_users) + 1, dtype=np.int64)
+    for u, h in user_his.items():
+        if not 0 <= int(u) < n_users:
+            raise ValueError(f"history_csr: user {u} outside [0, {n_users})")
+        ptr[int(u) + 1] = len(h)
+    ptr = np.cumsum(ptr)
+    items = np.zeros(int(ptr[-1]), dtype=np.int64)
+    for u, h in user_his.items():
+        if len(h):
+            items[ptr[int(u)]:ptr[int(u) + 1]] = np.fromiter((x[0] for x in h), dtype=np.int64, count=len(h))
+    return ptr, items
+
+
+def history_width(positions, history_max: int) -> int:
+    """the fixed padded width of device-collated histories: min(H, max position), or max position when H <= 0"""
+    import numpy as np
+    top = int(np.max(positions)) if len(positions) else 1
+    return max(1, min(int(history_max), top) if int(history_max) > 0 else top)
+
+
+class DeviceHistory:
+    """The inputs of b2r_collate_history for one SequentialModel training set, on the device: the history CSR of
+    ``corpus.user_his`` (``history_csr``) and the dataset's ``position`` column.  Every row's position is checked once,
+    here, to lie in [1, len(user_his[u])]; ``width`` (``history_width``) is the padded history width of every batch."""
+
+    def __init__(self, user_his: dict, n_users: int, users, positions, history_max: int, device):
+        import numpy as np
+        users = np.asarray(users, dtype=np.int64)
+        positions = np.asarray(positions, dtype=np.int64)
+        ptr, items = history_csr(user_his, n_users)
+        if users.shape != positions.shape:
+            raise ValueError("DeviceHistory: users and positions differ in length")
+        if len(users) and (users.min() < 0 or users.max() >= n_users):
+            raise ValueError("DeviceHistory: a training row's user is outside [0, n_users)")
+        have = ptr[users + 1] - ptr[users]
+        bad = np.flatnonzero((positions < 1) | (positions > have))
+        if len(bad):
+            r = int(bad[0])
+            raise ValueError(f"DeviceHistory: {len(bad)} training row(s) with a position outside [1, len(user_his[u])] "
+                             f"(first: row {r}, user {int(users[r])}, position {int(positions[r])}, history {int(have[r])})")
+        self.n_users, self.history_max = int(n_users), int(history_max)
+        self.width = history_width(positions, history_max)
+        self.ptr = torch.from_numpy(ptr).to(device)
+        self.items = torch.from_numpy(items if len(items) else np.zeros(1, dtype=np.int64)).to(device)
+        self.positions = torch.from_numpy(positions).to(device)
+
+    def collate(self, users: torch.Tensor, perm: Optional[torch.Tensor], start: int, Bn: int, out_hist: torch.Tensor,
+                out_len: torch.Tensor) -> None:
+        collate_history(users, self.positions, self.ptr, self.items, self.n_users, perm, start, Bn, self.history_max,
+                        out_hist, out_len)
+
+
+def collate_history(users: torch.Tensor, positions: torch.Tensor, his_ptr: torch.Tensor, his_items: torch.Tensor,
+                    n_users: int, perm: Optional[torch.Tensor], start: int, Bn: int, history_max: int,
+                    out_hist: torch.Tensor, out_len: torch.Tensor) -> None:
+    """b2r_collate_history: the history part of one SequentialModel training batch assembled on the device
+    (BaseModel.py:236-245,135-152), right-padded with 0 to out_hist's width Lp.  Bad rows are clamped and counted in the
+    out-of-range counter (check_ids raises IndexError)."""
+    _need_cuda(users, positions, his_ptr, his_items, perm, out_hist, out_len)
+    if out_hist.dim() != 2 or out_hist.shape[0] < Bn or out_len.numel() < Bn or his_ptr.numel() != int(n_users) + 1:
+        raise ValueError("collate_history: output buffers do not fit the batch")
+    for t in (users, positions, his_ptr, his_items, out_hist, out_len):
+        if t.dtype != torch.int64 or not t.is_contiguous():
+            raise TypeError("collate_history: contiguous int64 tensors expected")
+    if perm is not None and (perm.dtype != torch.int64 or not perm.is_contiguous()):
+        raise TypeError("collate_history: perm must be contiguous int64")
+    _lib.check(_lib.load().b2r_collate_history(_p(users), _p(positions), _p(his_ptr), _p(his_items), int(n_users), _p(perm),
+                                               int(start), int(Bn), int(history_max), int(out_hist.shape[1]), _p(out_hist),
+                                               _p(out_len), _p(err_flag(users.device)), _stream()), "b2r_collate_history")
+
+
 def adam_exact_advance(W: torch.Tensor, m: torch.Tensor, v: torch.Tensor, last: torch.Tensor, upto: int, opt,
                        rows: Optional[torch.Tensor] = None, stamp: int = 0, state_ld: int = 0) -> None:
     """Groundwork for the exact dense-Adam mode (b2r_adam_exact_advance): bring the listed unique rows (all rows when

@@ -7,8 +7,8 @@ What it does (SURVEY.md section 8b1): puts the reference ``src/`` on ``sys.path`
 reference still uses (np.object / np.int / np.float), imports the reference's model modules, builds classes
 that graft this package's kernel mixins onto the reference's own ``GeneralModel`` / ``SequentialModel`` (so the
 reference's Dataset, reader, runner, argument plumbing and checkpoint code are the ones that run), replaces
-``models.general.BPRMF.BPRMF`` etc. with them, and ``runpy``s ``main.py``.  With ``--fused_step 1`` or
-``--device_metrics 1`` on the command line it also registers ``helpers.B200Runner`` (a subclass of the reference's own
+``models.general.BPRMF.BPRMF`` etc. with them, and ``runpy``s ``main.py``.  With ``--fused_step 1``,
+``--device_metrics 1`` or ``--device_batches N`` on the command line it also registers ``helpers.B200Runner`` (a subclass of the reference's own
 BaseRunner) through the same by-name discovery.  Needs a CUDA device for the first forward call; there is no CPU
 fallback.  ``--ref`` defaults to the unmodified copy build() stages in oracle/_ref/src (oracle/stage_reference.py).
 """
@@ -28,7 +28,9 @@ def _make_runner_module(ref_runner_cls):
     (``main.py:164-176`` resolves the runner by the model's ``runner`` attribute and lets it add arguments):
       --fused_step 1      fit() = one C call per batch (model.train_step: forward, loss, backward, row-sparse optimizer;
                           next batch's index plan prefetched) instead of the loop body of BaseRunner.py:185-207;
-      --device_metrics 1  evaluate() ranks on the GPU (model.eval_ranks) instead of shipping predictions to the host.
+      --device_metrics 1  evaluate() ranks on the GPU (model.eval_ranks) instead of shipping predictions to the host;
+      --device_batches N  fit() = the epoch's negatives, row shuffle and collate (SASRec's histories included) as device
+                          kernels, seed N (runner.BaseRunner.fit_on_device) on the reference's own Dataset and corpus.
     Without those flags every method is the reference's."""
     import types
 
@@ -43,15 +45,21 @@ def _make_runner_module(ref_runner_cls):
                                 help="1 (with --table_mode fused): one C call per training step (model.train_step)")
             parser.add_argument("--device_metrics", type=int, default=0,
                                 help="1: rank the ground truth on the GPU (model.eval_ranks)")
+            parser.add_argument("--device_batches", type=int, default=0,
+                                help="non-zero (a value > 1 is the seed): negatives, row shuffle and collate of every "
+                                     "training batch on the GPU (runner.fit_on_device)")
             return parser
 
         def __init__(self, args):
             super().__init__(args)
             self.fused_step = getattr(args, "fused_step", 0)
             self.device_metrics = getattr(args, "device_metrics", 0)
+            self.device_batches = getattr(args, "device_batches", 0)
 
         def fit(self, dataset, epoch=-1):
             model = dataset.model
+            if self.device_batches:
+                return ours.BaseRunner.fit_on_device(self, dataset, epoch)
             if (self.fused_step and hasattr(model, "train_step")
                     and isinstance(model.optimizer, RowSparseOptimizer)):       # the lazily-built fused optimizer
                 dataset.actions_before_epoch()                                  # BaseRunner.py:178: negatives
@@ -185,8 +193,8 @@ def main(argv=None):
         del argv[i:i + 2]
     # the runner seams only matter when one of their flags is on the command line; otherwise the reference's own
     # BaseRunner class is the one main.py instantiates
-    want_runner = any(a in ("--fused_step", "--device_metrics") or a.startswith(("--fused_step=", "--device_metrics="))
-                      for a in argv)
+    flags = ("--fused_step", "--device_metrics", "--device_batches")
+    want_runner = any(a in flags or a.startswith(tuple(f + "=" for f in flags)) for a in argv)
     install(ref, b200_runner=want_runner)
     sys.argv = [os.path.join(ref, "main.py")] + argv
     runpy.run_path(os.path.join(ref, "main.py"), run_name="__main__")

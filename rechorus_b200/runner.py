@@ -81,7 +81,8 @@ class BaseRunner:
                                  "as BaseModel.py:206-214, counter-based stream)")
         parser.add_argument("--device_batches", type=int, default=0,
                             help="non-zero (a value > 1 is the seed): the whole epoch's batch production on the GPU -- "
-                                 "negatives, row shuffle and collate as device kernels (runner.fit_on_device; GeneralModel)")
+                                 "negatives, row shuffle and collate (histories included) as device kernels "
+                                 "(runner.fit_on_device); with --graph_step 1 the full-size batches replay one captured step")
         parser.add_argument("--device_metrics", type=int, default=0,
                             help="1: rank the ground truth on the GPU (model.eval_ranks) instead of copying predictions "
                                  "to the host for evaluate_method")
@@ -263,13 +264,21 @@ class BaseRunner:
         becomes three device operations: ``b2r_sample_negatives`` (one Philox draw + one binary search per negative, the
         reference's distribution from a counter-based stream), a device permutation, and ``b2r_collate_general`` per
         batch.  The training step is the model's ``train_step`` (one C call) or, for models without one, the plugin
-        contract's forward / loss / backward / optimizer.step on the device batch.  GeneralModel datasets only (a
-        SequentialModel needs the history CSR on the device too).  RNG: the host streams of the reference are NOT
-        reproduced (a sequential NumPy / torch CPU stream cannot be drawn in parallel); results are reproducible from
-        (seed, epoch)."""
+        contract's forward / loss / backward / optimizer.step on the device batch.
+
+        Sequential datasets (models with ``history_max``, e.g. SASRec) also get ``history_items [B, Lp]`` and ``lengths
+        [B]`` from ``b2r_collate_history`` (the slice of BaseModel.py:236-245 out of a device CSR of ``corpus.user_his``,
+        ops.DeviceHistory).  Every batch is right-padded to the fixed width Lp = min(history_max, max position), not to
+        the batch maximum as collate_batch does: the extra padding is dead work for SASRec (exact), and every full batch
+        has the same shape.  ``history_times`` is not produced; no kernel-backed model reads it.
+
+        ``--graph_step 1`` with a model without ``train_step`` (NeuMF, SASRec): the full-size batches are replayed through
+        one captured step (rechorus_b200.graph.GraphedStep), each collated straight into the captured inputs just before
+        its replay; the first full batch trains through the capture's warm-up step, the ragged last batch eagerly.
+
+        RNG: the host streams of the reference are NOT reproduced (a sequential NumPy / torch CPU stream cannot be drawn
+        in parallel); results are reproducible from (seed, epoch)."""
         model = dataset.model
-        if hasattr(model, "history_max"):
-            raise ValueError("fit_on_device: sequential datasets are not supported (history collate is host-side)")
         if model.optimizer is None:
             model.optimizer = self._build_optimizer(model)
         dev = model.device
@@ -281,6 +290,9 @@ class BaseRunner:
                   "items": torch.as_tensor(np.asarray(dataset.data["item_id"], dtype=np.int64)).to(dev),
                   "sampler": ops.DeviceNegativeSampler(corpus.train_clicked_set, corpus.n_users, corpus.n_items, dev, seed=seed),
                   "gen": torch.Generator(device=dev), "seed": seed, "epoch": 0}
+            if hasattr(model, "history_max"):
+                st["history"] = ops.DeviceHistory(corpus.user_his, corpus.n_users, dataset.data["user_id"],
+                                                  dataset.data["position"], model.history_max, dev)
             dataset.__dict__["_b2r_dev"] = st
         st["epoch"] += 1
         N, K, B = st["users"].numel(), int(model.num_neg), int(self.batch_size)
@@ -289,38 +301,75 @@ class BaseRunner:
         perm = torch.randperm(N, device=dev, generator=st["gen"])
         model.train()
         use_step = hasattr(model, "train_step") and isinstance(model.optimizer, RowSparseOptimizer)
+        use_graph = (not use_step and bool(getattr(self, "graph_step", 0))
+                     and isinstance(model.optimizer, RowSparseOptimizer))
+        his = st.get("history")
         n_steps = (N + B - 1) // B
         NB = 3                                                                       # batch buffers: current, next, one being refilled
+
+        def new_buf():
+            buf = {"user_id": torch.empty(B, dtype=torch.int64, device=dev),
+                   "item_id": torch.empty((B, K + 1), dtype=torch.int64, device=dev), "batch_size": B, "phase": "train"}
+            if his is not None:
+                buf["history_items"] = torch.empty((B, his.width), dtype=torch.int64, device=dev)
+                buf["lengths"] = torch.empty(B, dtype=torch.int64, device=dev)
+            return buf
+
         bufs = st.get("bufs")
         if bufs is None or bufs[0]["item_id"].shape != (B, K + 1):
-            bufs = st["bufs"] = [{"user_id": torch.empty(B, dtype=torch.int64, device=dev),
-                                  "item_id": torch.empty((B, K + 1), dtype=torch.int64, device=dev),
-                                  "batch_size": B, "phase": "train"} for _ in range(NB)]
+            bufs = st["bufs"] = [new_buf() for _ in range(NB)]
+
+        def fill(buf, k, Bn):
+            # two launches: user / candidate columns, then (sequential models) the history
+            ops.collate_general(st["users"], st["items"], neg, perm, k * B, Bn, buf["user_id"], buf["item_id"])
+            if his is not None:
+                his.collate(st["users"], perm, k * B, Bn, buf["history_items"], buf["lengths"])
 
         def batch(k):
             Bn = min(B, N - k * B)
             buf = bufs[k % NB]
-            ops.collate_general(st["users"], st["items"], neg, perm, k * B, Bn, buf["user_id"], buf["item_id"])
+            fill(buf, k, Bn)
             if Bn == B:
                 return buf
-            return {"user_id": buf["user_id"][:Bn], "item_id": buf["item_id"][:Bn], "batch_size": Bn, "phase": "train"}
+            out = {key: (v[:Bn] if isinstance(v, torch.Tensor) else v) for key, v in buf.items()}
+            out["batch_size"] = Bn
+            return out
+
+        def eager_step(feed):
+            model.optimizer.zero_grad()
+            loss = model.loss(model(feed))
+            loss.backward()
+            model.optimizer.step()
+            return loss.detach()
 
         losses = []
         ops.bprmf_step_reset()
         try:
-            cur = batch(0)
-            for k in range(n_steps):
-                nxt = batch(k + 1) if k + 1 < n_steps else None
-                if use_step:
-                    same = nxt is not None and nxt["item_id"].shape == cur["item_id"].shape
-                    losses.append(model.train_step(cur, nxt if same else None))
-                else:
-                    model.optimizer.zero_grad()
-                    loss = model.loss(model(cur))
-                    loss.backward()
-                    model.optimizer.step()
-                    losses.append(loss.detach())
-                cur = nxt
+            if use_graph:
+                from .graph import GraphedStep
+                gs = model.__dict__.get("_b2r_graphed_step")
+                for k in range(n_steps):
+                    if N - k * B < B:
+                        losses.append(eager_step(batch(k)))                         # the ragged last batch
+                    elif gs is None or not gs.matches(bufs[0]):
+                        gs = GraphedStep(model, batch(k), warmup=1)                 # its warm-up step IS this batch's step
+                        model.__dict__["_b2r_graphed_step"] = gs
+                        losses.append(gs.warmup_losses[0])
+                    else:
+                        # straight into the captured inputs; on the same stream, so after the previous replay read them
+                        fill(gs.static, k, B)
+                        losses.append(gs.replay().clone())
+                model.optimizer.sync_clock()                                       # the host step counter follows the device clock
+            else:
+                cur = batch(0)
+                for k in range(n_steps):
+                    nxt = batch(k + 1) if k + 1 < n_steps else None
+                    if use_step:
+                        same = nxt is not None and nxt["item_id"].shape == cur["item_id"].shape
+                        losses.append(model.train_step(cur, nxt if same else None))
+                    else:
+                        losses.append(eager_step(cur))
+                    cur = nxt
         finally:
             ops.bprmf_step_reset()
         out = float(torch.stack(losses).mean().cpu()) if losses else float("nan")
