@@ -457,6 +457,58 @@ B2R_API int b2r_rank_all_items(const float* Q, int ldq, const float* I, const in
                                int64_t* rank, int32_t* err_flag, b2r_stream_t stream);
 
 /* ------------------------------------------------------------------------------------------------
+ * Top-k recommendation lists (row a11): the TopK branch of save_rec_results (main.py:117-132) on the device.
+ *
+ * Ordering contract -- each row's list equals Python's stable sorted(zip(item_id, pred), key=score, reverse=True)[:k]:
+ *   - score descending, ties by candidate column ascending.  Candidate (score s, column c) becomes the 64-bit key
+ *     (~mono(s) << 32) | c, mono() the order-preserving map of the float bits to uint32; ascending key order is the
+ *     output order.  It is a total order, so results do not depend on grid or scheduling;
+ *   - -0.0 is canonicalised to +0.0 before the key is built (the two compare equal in Python);
+ *   - -inf (masked entries) sorts after every finite score, in column order; NaN sorts last, after -inf (Python's
+ *     result is undefined there);
+ *   - each row returns k' = min(k, C) entries, C the candidate count (1 + K, or n_items under test_all, where the list
+ *     [target] + arange(1, n_items) has n_items columns).  1 <= k <= 1024; larger k is B2R_E_UNSUPPORTED, as is
+ *     C >= 2^31 - 1.
+ *
+ * Clicked sets are a CSR over users: clicked_ptr int64 [n_users + 1], clicked_items int64, user u's items at
+ * clicked_items[clicked_ptr[u] .. clicked_ptr[u + 1]), sorted ascending without duplicates (b2r_topk_all_items
+ * binary-searches them; b2r_mask_clicked does not need the order).  For save_rec_results that is
+ * train_clicked_set[u] | residual_clicked_set[u] (BaseRunner.py:244-251).
+ *
+ * b2r_topk_rows:      top-k' of each row of pred [N, C] (row stride ld): out_idx int64 [N, k'] candidate columns,
+ *                     out_score float32 [N, k'] the scores as pred holds them (bit for bit).  A row of C <= 4096
+ *                     columns is one CTA (one warp when C <= 1024); a longer row is split into ranges of at least 4096 columns (at most
+ *                     ceil(1024 / N) of them), each range's top-k goes to the workspace and a second pass merges them.
+ *                     Workspace: b2r_topk_rows_workspace_bytes(N, C, k) (0 when rows are not split).
+ * b2r_mask_clicked:   pred[b*ld + j] = -inf for every clicked item j of user users[b] with 1 <= j < C: the test_all
+ *                     masking of BaseRunner.py:244-251 (column j is item j; column 0, the target, is never masked).
+ *                     Users outside [0, n_users) are counted in err_flag and their rows left as they are.
+ * b2r_topk_all_items: the test_all protocol fused -- candidates [target] + arange(1, n_items) scored <Q[b], I[j]>,
+ *                     clicked items masked as b2r_mask_clicked does, top-k' by the contract above -- without the
+ *                     [B, n_items] score matrix.  Q [B, ldq] query rows, I [n_items, d], target [B], users [B].
+ *                     out_items int64 [B, k'] item ids (column 0 reports target[b]), out_scores float32 [B, k'].
+ *                     Items are scored in chunks of W columns (W = 32 MB / (4 B), a multiple of 128 in [128, 8192])
+ *                     into the workspace, and each chunk is merged into a running top-k list per row; workspace
+ *                     b2r_topk_all_items_workspace_bytes(B, n_items, k) = B * (4 W + 8 k + 8) bytes rounded up,
+ *                     independent of n_items once n_items exceeds W.  Scores are accumulated s = fmaf(q_k, i_k, s) for
+ *                     k ascending, as b2r_rank_all_items does, so a row whose rank r <= k has no exact ties puts its
+ *                     target at position r; they can differ in the last bit from b2r_rowdot_fwd's.  Scores are
+ *                     returned from the keys: a -0.0 score comes back as +0.0 and every NaN as 0x7fc00000.  Bad target
+ *                     or user ids are clamped to 0 and counted in err_flag.
+ * ---------------------------------------------------------------------------------------------- */
+B2R_API size_t b2r_topk_rows_workspace_bytes(int64_t N, int64_t C, int k);
+B2R_API int b2r_topk_rows(const float* pred, int64_t N, int64_t C, int64_t ld, int k, int64_t* out_idx, float* out_score,
+                          void* workspace, size_t workspace_bytes, b2r_stream_t stream);
+B2R_API int b2r_mask_clicked(float* pred, int64_t N, int64_t C, int64_t ld, const int64_t* users,
+                             const int64_t* clicked_ptr, const int64_t* clicked_items, int64_t n_users, int32_t* err_flag,
+                             b2r_stream_t stream);
+B2R_API size_t b2r_topk_all_items_workspace_bytes(int B, int64_t n_items, int k);
+B2R_API int b2r_topk_all_items(const float* Q, int ldq, const float* I, int64_t n_items, int d, const int64_t* target,
+                               const int64_t* users, int B, const int64_t* clicked_ptr, const int64_t* clicked_items,
+                               int64_t n_users, int k, int64_t* out_items, float* out_scores, int32_t* err_flag,
+                               void* workspace, size_t workspace_bytes, b2r_stream_t stream);
+
+/* ------------------------------------------------------------------------------------------------
  * Fused BPRMF forward + loss + query-side backward: every candidate row is read from HBM once and stays in
  * registers between scoring and the gradient.  Outputs: grad_pred [B,C] (= d loss / d pred, loss = mean of the
  * per-sample losses), row_loss [B] (per-sample -log S), dQ [B,d] (= sum_c g[b,c] I[iid[b,c]]), pred [B,C]

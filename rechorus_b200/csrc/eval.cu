@@ -14,7 +14,9 @@
 // Every score on the test_all path is accumulated as s = fmaf(q_k, i_k, s) for k ascending -- in the GEMM tile, in
 // k_target_score and in k_rank_unmask alike -- so the same (b, j) always yields the same bits and the comparison
 // against s0 is consistent between the three kernels.  Counts are integers: atomics do not affect determinism.
+// The GEMM tile itself (rank_tile.cuh) is shared with topk.cu's b2r_topk_all_items.
 #include "common.cuh"
+#include "rank_tile.cuh"
 
 namespace b2r {
 
@@ -83,9 +85,6 @@ k_target_score(const float* __restrict__ Q, int ldq, const float* __restrict__ I
     rank[b] = 1;                                   // the candidate list's column 0 is the target itself
 }
 
-// 128 queries x 128 items per CTA, 256 threads, 8 x 8 scores per thread, the reduction dimension in chunks of 16.
-constexpr int kTQ = 128, kTI = 128, kTK = 16, kAT = 256;
-
 __global__ void __launch_bounds__(kAT)
 k_rank_all(const float* __restrict__ Q, int ldq, const float* __restrict__ I, const float* __restrict__ s0, int B,
            int64_t n_items, int d, unsigned long long* __restrict__ rank) {
@@ -96,64 +95,7 @@ k_rank_all(const float* __restrict__ Q, int ldq, const float* __restrict__ I, co
     const int q0 = blockIdx.y * kTQ;
     const int64_t j0 = (int64_t)blockIdx.x * kTI;
     float acc[8][8];
-#pragma unroll
-    for (int i = 0; i < 8; ++i)
-#pragma unroll
-        for (int j = 0; j < 8; ++j) acc[i][j] = 0.f;
-    // loader mapping: thread -> (row = tid % 128, 8 consecutive k of the 16-wide chunk): a warp stores 32 consecutive
-    // columns of one shared-memory row (conflict-free) and reads one full 32-byte sector per lane
-    const int lr = tid % kTQ, lk = (tid / kTQ) * 8;
-    for (int k0 = 0; k0 < d; k0 += kTK) {
-        {
-            const int q = q0 + lr;
-            float v[8];
-#pragma unroll
-            for (int i = 0; i < 8; ++i) v[i] = 0.f;
-            if (q < B) {
-#pragma unroll
-                for (int i = 0; i < 8; ++i)
-                    if (k0 + lk + i < d) v[i] = Q[(int64_t)q * ldq + k0 + lk + i];
-            }
-#pragma unroll
-            for (int i = 0; i < 8; ++i) Qs[lk + i][lr] = v[i];
-        }
-        {
-            const int64_t j = j0 + lr;
-            float v[8];
-#pragma unroll
-            for (int i = 0; i < 8; ++i) v[i] = 0.f;
-            if (j < n_items) {
-                if (k0 + lk + 8 <= d) {
-                    const float4 a = ld_row4(I + j * d + k0 + lk);
-                    const float4 c = ld_row4(I + j * d + k0 + lk + 4);
-                    v[0] = a.x; v[1] = a.y; v[2] = a.z; v[3] = a.w;
-                    v[4] = c.x; v[5] = c.y; v[6] = c.z; v[7] = c.w;
-                } else {
-#pragma unroll
-                    for (int i = 0; i < 8; ++i)
-                        if (k0 + lk + i < d) v[i] = I[j * d + k0 + lk + i];
-                }
-            }
-#pragma unroll
-            for (int i = 0; i < 8; ++i) Is[lk + i][lr] = v[i];
-        }
-        __syncthreads();
-#pragma unroll
-        for (int kk = 0; kk < kTK; ++kk) {
-            // k beyond d contributes fmaf(0, 0, acc) == acc exactly, so a ragged last chunk does not change the bits
-            const float4 a0 = *reinterpret_cast<const float4*>(&Qs[kk][ty * 8]);
-            const float4 a1 = *reinterpret_cast<const float4*>(&Qs[kk][ty * 8 + 4]);
-            const float4 b0 = *reinterpret_cast<const float4*>(&Is[kk][tx * 8]);
-            const float4 b1 = *reinterpret_cast<const float4*>(&Is[kk][tx * 8 + 4]);
-            const float av[8] = {a0.x, a0.y, a0.z, a0.w, a1.x, a1.y, a1.z, a1.w};
-            const float bv[8] = {b0.x, b0.y, b0.z, b0.w, b1.x, b1.y, b1.z, b1.w};
-#pragma unroll
-            for (int i = 0; i < 8; ++i)
-#pragma unroll
-                for (int j = 0; j < 8; ++j) acc[i][j] = fmaf(av[i], bv[j], acc[i][j]);
-        }
-        __syncthreads();
-    }
+    rank_tile_accumulate(Q, ldq, I, B, n_items, d, q0, j0, Qs, Is, acc);
     // epilogue: compare against the target's score and count; item 0 is not a candidate (ids are 1-based)
 #pragma unroll
     for (int i = 0; i < 8; ++i) {

@@ -152,6 +152,15 @@ SIGNATURES = {
     "b2r_rank_histogram": (C.c_int, [C.c_void_p, C.c_int64, C.c_int, C.c_void_p, C.c_void_p]),
     "b2r_rank_all_items": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_int, C.c_int64, C.c_int,
                                      C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "b2r_topk_rows_workspace_bytes": (C.c_size_t, [C.c_int64, C.c_int64, C.c_int]),
+    "b2r_topk_rows": (C.c_int, [C.c_void_p, C.c_int64, C.c_int64, C.c_int64, C.c_int, C.c_void_p, C.c_void_p,
+                                C.c_void_p, C.c_size_t, C.c_void_p]),
+    "b2r_mask_clicked": (C.c_int, [C.c_void_p, C.c_int64, C.c_int64, C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p,
+                                   C.c_int64, C.c_void_p, C.c_void_p]),
+    "b2r_topk_all_items_workspace_bytes": (C.c_size_t, [C.c_int, C.c_int64, C.c_int]),
+    "b2r_topk_all_items": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p, C.c_int64, C.c_int, C.c_void_p, C.c_void_p,
+                                     C.c_int, C.c_void_p, C.c_void_p, C.c_int64, C.c_int, C.c_void_p, C.c_void_p,
+                                     C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p]),
     "b2r_bucket_apply_pair": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_void_p]),
     "b2r_adam_exact_advance": (C.c_int, [C.c_void_p, C.c_int64, C.c_int64, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p,
                                          C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p]),

@@ -242,22 +242,114 @@ def rank_all_items(q: torch.Tensor, table: torch.Tensor, target: torch.Tensor,
     return rank
 
 
+def clicked_csr(sets: Sequence[dict], n_users: int):
+    """The union of per-user item sets ({user: iterable of item ids}, e.g. corpus.train_clicked_set) as a CSR over
+    users: ptr int64 [n_users + 1] and items int64 (at least one slot), user u's items sorted ascending without
+    duplicates at items[ptr[u]:ptr[u + 1]].  Users outside [0, n_users) are ignored.  NumPy arrays."""
+    import numpy as np
+    parts = {}
+    for s in sets:
+        for u, items in s.items():
+            if 0 <= int(u) < n_users and len(items):
+                parts.setdefault(int(u), []).append(np.fromiter(items, dtype=np.int64, count=len(items)))
+    rows = {u: (np.unique(np.concatenate(p)) if len(p) > 1 else np.sort(p[0])) for u, p in parts.items()}
+    ptr = np.zeros(int(n_users) + 1, dtype=np.int64)
+    for u, r in rows.items():
+        ptr[u + 1] = len(r)
+    ptr = np.cumsum(ptr)
+    flat = np.zeros(max(int(ptr[-1]), 1), dtype=np.int64)
+    for u, r in rows.items():
+        flat[ptr[u]:ptr[u + 1]] = r
+    return ptr, flat
+
+
+class ClickedSets:
+    """The items BaseRunner.py:244-251 masks under test_all -- train_clicked_set[u] | residual_clicked_set[u] -- as a
+    device CSR (clicked_csr): the input of mask_clicked and topk_all_items."""
+
+    def __init__(self, train_clicked_set: dict, residual_clicked_set: dict, n_users: int, device):
+        ptr, items = clicked_csr([train_clicked_set, residual_clicked_set], n_users)
+        self.n_users = int(n_users)
+        self.ptr = torch.from_numpy(ptr).to(device)
+        self.items = torch.from_numpy(items).to(device)
+
+
+def _topk_k(k: int) -> int:
+    k = int(k)
+    if not 1 <= k <= 1024:
+        raise ValueError(f"top-k lists support 1 <= k <= 1024, got k={k}")
+    return k
+
+
+def topk_rows(pred: torch.Tensor, k: int) -> Tuple[torch.Tensor, torch.Tensor]:
+    """Top-k' (k' = min(k, C)) of every row of pred [N, C] in the order of Python's stable
+    sorted(..., key=score, reverse=True) (include/b200rec.h): (columns int64 [N, k'], scores float32 [N, k'])."""
+    _need_cuda(pred)
+    pred = _f32c(pred, "pred")
+    if pred.dim() != 2 or pred.shape[1] < 1:
+        raise ValueError("topk_rows: pred must be [N, C] with C >= 1")
+    k = _topk_k(k)
+    N, Cn = pred.shape
+    kk = min(k, Cn)
+    idx = torch.empty((N, kk), dtype=torch.int64, device=pred.device)
+    val = torch.empty((N, kk), dtype=torch.float32, device=pred.device)
+    L = _lib.load()
+    nb = L.b2r_topk_rows_workspace_bytes(N, Cn, k)
+    ws = _ws(nb, pred.device) if nb else None
+    _lib.check(L.b2r_topk_rows(_p(pred), N, Cn, Cn, k, _p(idx), _p(val), _p(ws), nb, _stream()), "b2r_topk_rows")
+    return idx, val
+
+
+def mask_clicked(pred: torch.Tensor, users: torch.Tensor, clicked: ClickedSets) -> torch.Tensor:
+    """pred[b, j] = -inf in place for every item j the user users[b] clicked, 1 <= j < C (BaseRunner.py:244-251 for
+    the test_all candidate list, where column j is item j).  Returns pred."""
+    _need_cuda(pred, users, clicked.ptr)
+    if pred.dtype != torch.float32 or not pred.is_contiguous() or pred.dim() != 2:
+        raise TypeError("mask_clicked: pred must be a contiguous float32 [N, C] tensor")
+    users = _i64c(users.reshape(-1), "users")
+    if users.numel() != pred.shape[0]:
+        raise ValueError("mask_clicked: one user per row")
+    N, Cn = pred.shape
+    _lib.check(_lib.load().b2r_mask_clicked(_p(pred), N, Cn, Cn, _p(users), _p(clicked.ptr), _p(clicked.items),
+                                            clicked.n_users, _p(err_flag(pred.device)), _stream()), "b2r_mask_clicked")
+    return pred
+
+
+def topk_all_items(q: torch.Tensor, table: torch.Tensor, target: torch.Tensor, users: torch.Tensor,
+                   clicked: ClickedSets, k: int) -> Tuple[torch.Tensor, torch.Tensor]:
+    """The test_all top-k' lists (k' = min(k, n_items)) of dot-product models without the [B, n_items] scores:
+    candidates [target] + arange(1, n_items) scored <q[b], table[j]>, clicked items masked (-inf), ordered as
+    topk_rows orders them.  Returns (item ids int64 [B, k'], scores float32 [B, k'])."""
+    _need_cuda(q, table, target, users, clicked.ptr)
+    q, table = _f32c(q, "q"), _f32c(table, "table")
+    target, users = _i64c(target.reshape(-1), "target"), _i64c(users.reshape(-1), "users")
+    if q.dim() != 2 or table.dim() != 2 or q.shape[1] != table.shape[1] or target.numel() != q.shape[0] \
+            or users.numel() != q.shape[0]:
+        raise ValueError("topk_all_items: q [B, d], table [n_items, d], target [B], users [B]")
+    k = _topk_k(k)
+    B, d = q.shape
+    n_items = table.shape[0]
+    kk = min(k, n_items)
+    items = torch.empty((B, kk), dtype=torch.int64, device=q.device)
+    scores = torch.empty((B, kk), dtype=torch.float32, device=q.device)
+    if B == 0:
+        return items, scores
+    L = _lib.load()
+    nb = L.b2r_topk_all_items_workspace_bytes(B, n_items, k)
+    ws = _ws(nb, q.device)
+    _lib.check(L.b2r_topk_all_items(_p(q), d, _p(table), n_items, d, _p(target), _p(users), B, _p(clicked.ptr),
+                                    _p(clicked.items), clicked.n_users, k, _p(items), _p(scores),
+                                    _p(err_flag(q.device)), _p(ws), nb, _stream()), "b2r_topk_all_items")
+    return items, scores
+
+
 class DeviceNegativeSampler:
     """Groundwork for SURVEY.md §8 f3: models/BaseModel.py:206-214 on the device.  Holds the training clicks as a CSR
     on the GPU and draws ``num_neg`` non-clicked items per training row with b2r_sample_negatives.  Same distribution
     as the reference's NumPy loop, a different (counter-based, reproducible from (seed, epoch)) random stream."""
 
     def __init__(self, train_clicked_set: dict, n_users: int, n_items: int, device, seed: int = 0):
-        import numpy as np
-        ptr = np.zeros(n_users + 1, dtype=np.int64)
-        for u, items in train_clicked_set.items():
-            if 0 <= int(u) < n_users:
-                ptr[int(u) + 1] = len(items)
-        ptr = np.cumsum(ptr)
-        flat = np.zeros(max(int(ptr[-1]), 1), dtype=np.int64)
-        for u, items in train_clicked_set.items():
-            if 0 <= int(u) < n_users and len(items):
-                flat[ptr[int(u)]:ptr[int(u) + 1]] = np.sort(np.fromiter(items, dtype=np.int64, count=len(items)))
+        ptr, flat = clicked_csr([train_clicked_set], n_users)
         self.ptr = torch.from_numpy(ptr).to(device)
         self.items = torch.from_numpy(flat).to(device)
         self.n_users, self.n_items, self.seed = int(n_users), int(n_items), int(seed)

@@ -8,7 +8,7 @@ reference still uses (np.object / np.int / np.float), imports the reference's mo
 that graft this package's kernel mixins onto the reference's own ``GeneralModel`` / ``SequentialModel`` (so the
 reference's Dataset, reader, runner, argument plumbing and checkpoint code are the ones that run), replaces
 ``models.general.BPRMF.BPRMF`` etc. with them, and ``runpy``s ``main.py``.  With ``--fused_step 1``,
-``--device_metrics 1`` or ``--device_batches N`` on the command line it also registers ``helpers.B200Runner`` (a subclass of the reference's own
+``--device_metrics 1``, ``--device_batches N`` or ``--device_rec 1`` on the command line it also registers ``helpers.B200Runner`` (a subclass of the reference's own
 BaseRunner) through the same by-name discovery.  Needs a CUDA device for the first forward call; there is no CPU
 fallback.  ``--ref`` defaults to the unmodified copy build() stages in oracle/_ref/src (oracle/stage_reference.py).
 """
@@ -30,7 +30,9 @@ def _make_runner_module(ref_runner_cls):
                           next batch's index plan prefetched) instead of the loop body of BaseRunner.py:185-207;
       --device_metrics 1  evaluate() ranks on the GPU (model.eval_ranks) instead of shipping predictions to the host;
       --device_batches N  fit() = the epoch's negatives, row shuffle and collate (SASRec's histories included) as device
-                          kernels, seed N (runner.BaseRunner.fit_on_device) on the reference's own Dataset and corpus.
+                          kernels, seed N (runner.BaseRunner.fit_on_device) on the reference's own Dataset and corpus;
+      --device_rec 1      the final top-100 lists of save_rec_results (main.py:117-132, TopK mode) computed on the GPU
+                          (runner.BaseRunner.recommend) and written by runner.BaseRunner.save_rec_results.
     Without those flags every method is the reference's."""
     import types
 
@@ -48,6 +50,9 @@ def _make_runner_module(ref_runner_cls):
             parser.add_argument("--device_batches", type=int, default=0,
                                 help="non-zero (a value > 1 is the seed): negatives, row shuffle and collate of every "
                                      "training batch on the GPU (runner.fit_on_device)")
+            parser.add_argument("--device_rec", type=int, default=0,
+                                help="1: compute the final top-k recommendation lists of save_rec_results on the GPU "
+                                     "(TopK mode; the CSV is written on the host, byte-identical in format)")
             return parser
 
         def __init__(self, args):
@@ -55,6 +60,9 @@ def _make_runner_module(ref_runner_cls):
             self.fused_step = getattr(args, "fused_step", 0)
             self.device_metrics = getattr(args, "device_metrics", 0)
             self.device_batches = getattr(args, "device_batches", 0)
+            self.device_rec = getattr(args, "device_rec", 0)
+            if self.device_rec:
+                _install_device_rec()
 
         def fit(self, dataset, epoch=-1):
             model = dataset.model
@@ -72,9 +80,37 @@ def _make_runner_module(ref_runner_cls):
                 return ours.BaseRunner.evaluate_on_device(self, dataset, topks, metrics)
             return super().evaluate(dataset, topks, metrics)
 
+        recommend = ours.BaseRunner.recommend
+        save_rec_results = ours.BaseRunner.save_rec_results
+
     mod = types.ModuleType("helpers.B200Runner")
     mod.B200Runner = B200Runner
     return mod
+
+
+def _install_device_rec() -> None:
+    """Point the running main.py's module-level save_rec_results at the device route.  While runpy executes main.py it
+    is sys.modules["__main__"], and main() looks the function up in those globals at call time (main.py:91-93), so
+    main.py itself stays unmodified.  Only the TopK mode (--model_mode '' or TopK) is replaced; the CTR and
+    Impression branches, and models without the kernel mixins' ``recommend``, keep the reference's function."""
+    import logging
+    main_mod = sys.modules.get("__main__")
+    init_args = getattr(main_mod, "init_args", None)
+    ref_fn = getattr(main_mod, "save_rec_results", None)
+    if init_args is None or ref_fn is None or getattr(init_args, "model_mode", None) not in ("", "TopK"):
+        return
+
+    def save_rec_results(dataset, runner_, topk):
+        if not hasattr(dataset.model, "recommend"):                 # not a kernel-backed model: the reference's route
+            return ref_fn(dataset, runner_, topk)
+        # the result path of main.py:99-101
+        model_name = "{0}{1}".format(init_args.model_name, init_args.model_mode)
+        result_path = os.path.join(runner_.log_path, runner_.save_appendix, "rec-{}-{}.csv".format(model_name,
+                                                                                              dataset.phase))
+        logging.info("Saving top-{} recommendation results to: {}".format(topk, result_path))
+        runner_.save_rec_results(dataset, result_path, topk, sep=main_mod.args.sep)
+
+    main_mod.save_rec_results = save_rec_results
 
 
 def install(ref_src: str = DEFAULT_REF, b200_runner: bool = False):
@@ -193,7 +229,7 @@ def main(argv=None):
         del argv[i:i + 2]
     # the runner seams only matter when one of their flags is on the command line; otherwise the reference's own
     # BaseRunner class is the one main.py instantiates
-    flags = ("--fused_step", "--device_metrics", "--device_batches")
+    flags = ("--fused_step", "--device_metrics", "--device_batches", "--device_rec")
     want_runner = any(a in flags or a.startswith(tuple(f + "=" for f in flags)) for a in argv)
     install(ref, b200_runner=want_runner)
     sys.argv = [os.path.join(ref, "main.py")] + argv

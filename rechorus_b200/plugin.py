@@ -152,6 +152,35 @@ class _KernelModelMixin:
                 pred[mask_row, mask_item] = float("-inf")
             return ops.gt_rank(pred)
 
+    def has_query_rows(self) -> bool:
+        """whether this model scores candidates as dot products with item-table rows (query_rows is overridden)"""
+        return type(self).query_rows is not _KernelModelMixin.query_rows
+
+    def recommend(self, feed_dict: dict, k: int, clicked=None):
+        """The top-k' recommendation lists (k' = min(k, C)) of one evaluation batch on the device: (item ids int64 [B, k'],
+        scores float32 [B, k']) in the order of main.py:117-132's stable sort of (item_id, prediction) pairs
+        (include/b200rec.h).  Under test_all the candidates are [target] + arange(1, n_items) with the items of
+        ``clicked`` (ops.ClickedSets) masked to -inf (BaseRunner.py:244-251); column 0 of feed_dict["item_id"] is the
+        target and a dot-product model needs no other column (ops.topk_all_items scores the catalogue itself)."""
+        with torch.no_grad():
+            opt = self.__dict__.get("_b2r_optimizer")
+            if getattr(opt, "exact_dense", False) and not self.training:
+                opt.flush()                     # exact dense-Adam mode: lists must see rows advanced through skipped steps
+            item_id = feed_dict["item_id"]
+            test_all = bool(getattr(self, "test_all", 0))
+            if test_all and clicked is None:
+                raise ValueError("recommend under test_all needs the clicked sets (ops.ClickedSets) to mask")
+            if test_all and self.has_query_rows():
+                q, table = self.query_rows(feed_dict)
+                return ops.topk_all_items(q, table, item_id[:, 0], feed_dict["user_id"], clicked, k)
+            if test_all and item_id.shape[1] != self.item_num:
+                raise ValueError(f"test_all candidate lists have {self.item_num} columns, got {item_id.shape[1]}")
+            pred = self.forward(feed_dict)["prediction"].contiguous()
+            if test_all:
+                ops.mask_clicked(pred, feed_dict["user_id"], clicked)
+            cols, scores = ops.topk_rows(pred, k)
+            return item_id.gather(1, cols), scores
+
 
 class BPRMFKernels(_KernelModelMixin):
     """models/general/BPRMF.py:18-45 (BPRMFBase) on K1/K2."""

@@ -486,5 +486,71 @@ class BaseRunner:
             preds[rows, cols] = -np.inf
         return preds
 
+    def recommend(self, dataset, k: int = 100):
+        """The top-k' recommendation list of every row of an evaluation phase (main.py:117-132's TopK branch) computed on
+        the device: (users as dataset.data["user_id"] holds them, item ids int64 [N, k'], scores float32 [N, k']) as host
+        arrays, rows in dataset order.  Batches of eval_batch_size rows are built on the device, not by the DataLoader:
+        b2r_collate_general over the phase's fixed neg_items (uploaded once), the history slice of ops.DeviceHistory for
+        sequential models, and under test_all either nothing beyond the targets (dot-product models: ops.topk_all_items
+        scores the catalogue) or a [target | arange(1, n_items)] matrix (NeuMF) masked with ops.mask_clicked."""
+        model = dataset.model
+        model.eval()
+        dev = model.device
+        corpus, data = dataset.corpus, dataset.data
+        N, B = len(dataset), int(self.eval_batch_size)
+        users = torch.as_tensor(np.asarray(data["user_id"], dtype=np.int64)).to(dev)
+        targets = torch.as_tensor(np.asarray(data["item_id"], dtype=np.int64)).to(dev)
+        test_all = bool(model.test_all)
+        clicked = (ops.ClickedSets(corpus.train_clicked_set, corpus.residual_clicked_set, corpus.n_users, dev)
+                   if test_all else None)
+        his = None
+        if hasattr(model, "history_max"):
+            his = ops.DeviceHistory(corpus.user_his, corpus.n_users, data["user_id"], data["position"], model.history_max,
+                                    dev)
+            hist_buf = torch.empty((B, his.width), dtype=torch.int64, device=dev)
+            len_buf = torch.empty(B, dtype=torch.int64, device=dev)
+        if not test_all:
+            neg = torch.as_tensor(np.asarray(data["neg_items"], dtype=np.int64).reshape(N, -1)).to(dev)
+            uid_buf = torch.empty(B, dtype=torch.int64, device=dev)
+            iid_buf = torch.empty((B, neg.shape[1] + 1), dtype=torch.int64, device=dev)
+        elif not model.has_query_rows():
+            arange = torch.arange(1, corpus.n_items, dtype=torch.int64, device=dev)
+        out_items, out_scores = [], []
+        for start in range(0, N, B):
+            Bn = min(B, N - start)
+            feed = {"batch_size": Bn, "phase": dataset.phase}
+            if test_all:
+                tgt = targets[start:start + Bn].view(-1, 1)
+                feed["user_id"] = users[start:start + Bn]
+                feed["item_id"] = tgt if model.has_query_rows() else torch.cat([tgt, arange.expand(Bn, -1)], dim=1)
+            else:
+                ops.collate_general(users, targets, neg, None, start, Bn, uid_buf, iid_buf)
+                feed["user_id"], feed["item_id"] = uid_buf[:Bn], iid_buf[:Bn]
+            if his is not None:
+                his.collate(users, None, start, Bn, hist_buf, len_buf)
+                feed["history_items"], feed["lengths"] = hist_buf[:Bn], len_buf[:Bn]
+            items, scores = model.recommend(feed, k, clicked)
+            out_items.append(items)
+            out_scores.append(scores)
+        _poll_ids(model)
+        if not out_items:
+            return list(data["user_id"]), np.zeros((0, 0), np.int64), np.zeros((0, 0), np.float32)
+        return (list(data["user_id"]), torch.cat(out_items).cpu().numpy(), torch.cat(out_scores).cpu().numpy())
+
+    def save_rec_results(self, dataset, result_path: str, topk: int = 100, sep: str = "\t") -> None:
+        """The TopK branch of main.py:117-132 (save_rec_results) with the lists from ``recommend``: same columns and
+        element types (NumPy int64 item ids, NumPy float32 scores), so the CSV matches the reference's byte for byte.
+        Writing the CSV stays on the host."""
+        import pandas as pd
+        users, items, scores = self.recommend(dataset, topk)
+        d = os.path.dirname(result_path)
+        if d:
+            os.makedirs(d, exist_ok=True)
+        rec_df = pd.DataFrame(columns=["user_id", "rec_items", "rec_predictions"])
+        rec_df["user_id"] = users
+        rec_df["rec_items"] = [list(r) for r in items]
+        rec_df["rec_predictions"] = [list(r) for r in scores]
+        rec_df.to_csv(result_path, sep=sep, index=False)
+
     def print_res(self, dataset) -> str:
         return "(" + format_metric(self.evaluate(dataset, self.topk, self.metrics)) + ")"
