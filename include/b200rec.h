@@ -449,12 +449,23 @@ B2R_API int b2r_adam_exact_advance(const int64_t* rows, int64_t n, int64_t n_row
  *                     sequence states), (mask_row[e], mask_item[e]) the n_mask unique (batch row, item id) pairs to
  *                     exclude, s0 [B] scratch that receives the targets' scores.  The unmasked target column counts
  *                     (it scores equal to column 0), exactly as in the reference.
+ * b2r_rank_all_items_clicked: the same ranks with the masked pairs read from the clicked-item CSR of the top-k section
+ *                     below (clicked_ptr [n_users + 1], clicked_items; sorted, no duplicates): row b excludes every
+ *                     clicked item j of user users[b] with 1 <= j < n_items, i.e. the pairs BaseRunner.py:244-251 sets
+ *                     to -inf.  Each clicked item is scored by one thread with the fmaf order of the GEMM tile, so the
+ *                     ranks equal b2r_rank_all_items' with (mask_row, mask_item) listing the same pairs.  A user outside
+ *                     [0, n_users) is counted in err_flag and its row left unmasked; a bad target is clamped to 0 and
+ *                     counted.  s0 [B] is scratch as above.
  * ---------------------------------------------------------------------------------------------- */
 B2R_API int b2r_gt_rank(const float* pred, int64_t N, int64_t C, int64_t ld, int64_t* rank, b2r_stream_t stream);
 B2R_API int b2r_rank_histogram(const int64_t* rank, int64_t N, int kmax, int64_t* hist, b2r_stream_t stream);
 B2R_API int b2r_rank_all_items(const float* Q, int ldq, const float* I, const int64_t* target, int B, int64_t n_items,
                                int d, const int64_t* mask_row, const int64_t* mask_item, int64_t n_mask, float* s0,
                                int64_t* rank, int32_t* err_flag, b2r_stream_t stream);
+B2R_API int b2r_rank_all_items_clicked(const float* Q, int ldq, const float* I, int64_t n_items, int d,
+                                       const int64_t* target, const int64_t* users, int B, const int64_t* clicked_ptr,
+                                       const int64_t* clicked_items, int64_t n_users, float* s0, int64_t* rank,
+                                       int32_t* err_flag, b2r_stream_t stream);
 
 /* ------------------------------------------------------------------------------------------------
  * Top-k recommendation lists (row a11): the TopK branch of save_rec_results (main.py:117-132) on the device.

@@ -10,9 +10,11 @@
 //                    fp32 GEMM whose epilogue compares and counts instead of storing
 //   k_rank_unmask    rank[b] -= 1 for every listed (b, j) with <q_b, I[j]> >= s0[b]   the clicked-item masking
 //                    preds[rows, cols] = -inf of BaseRunner.py:244-251
+//   k_rank_unmask_clicked  the same masking read from the clicked-item CSR (b2r_mask_clicked's): one warp per batch row
+//                    walks users[b]'s slice, one lane scores one clicked item
 //
 // Every score on the test_all path is accumulated as s = fmaf(q_k, i_k, s) for k ascending -- in the GEMM tile, in
-// k_target_score and in k_rank_unmask alike -- so the same (b, j) always yields the same bits and the comparison
+// k_target_score and in both unmask kernels alike -- so the same (b, j) always yields the same bits and the comparison
 // against s0 is consistent between the three kernels.  Counts are integers: atomics do not affect determinism.
 // The GEMM tile itself (rank_tile.cuh) is shared with topk.cu's b2r_topk_all_items.
 #include "common.cuh"
@@ -133,9 +135,62 @@ k_rank_unmask(const float* __restrict__ Q, int ldq, const float* __restrict__ I,
     }
 }
 
+// One warp per batch row.  Each clicked item is scored by ONE lane with the scalar fmaf chain of k_target_score (k
+// ascending; the float4 loads only fetch four consecutive k at once), so its bits equal the GEMM tile's and s0's.  The
+// CSR holds each item once per user, so the count equals k_rank_unmask's over the same (row, item) pairs.  The warp is
+// the only writer of rank[b] here (k_rank_all has finished: same stream), so no atomic is needed.
+__global__ void __launch_bounds__(kRT)
+k_rank_unmask_clicked(const float* __restrict__ Q, int ldq, const float* __restrict__ I, const float* __restrict__ s0,
+                      const int64_t* __restrict__ users, const int64_t* __restrict__ clicked_ptr,
+                      const int64_t* __restrict__ clicked_items, int64_t n_users, int B, int64_t n_items, int d,
+                      int64_t* __restrict__ rank, int32_t* __restrict__ err_flag) {
+    const int lane = threadIdx.x % 32, warp = threadIdx.x / 32;
+    for (int64_t b = (int64_t)blockIdx.x * (kRT / 32) + warp; b < B; b += (int64_t)gridDim.x * (kRT / 32)) {
+        const int64_t u = users[b];
+        if (u < 0 || u >= n_users) {               // counted once; the row stays unmasked
+            if (lane == 0 && err_flag) atomicAdd(err_flag, 1);
+            continue;
+        }
+        const int64_t beg = clicked_ptr[u], end = clicked_ptr[u + 1];
+        const float* q = Q + b * ldq;
+        const float t = s0[b];
+        int cnt = 0;
+        for (int64_t e = beg + lane; e < end; e += 32) {
+            const int64_t j = clicked_items[e];
+            if (j < 1 || j >= n_items) continue;   // not a column of the candidate list
+            const float* it = I + j * d;
+            float s = 0.f;
+            for (int k = 0; k < d; k += 4) {
+                const float4 v = ld_row4(it + k);
+                s = fmaf(q[k], v.x, s);
+                s = fmaf(q[k + 1], v.y, s);
+                s = fmaf(q[k + 2], v.z, s);
+                s = fmaf(q[k + 3], v.w, s);
+            }
+            cnt += (s >= t) ? 1 : 0;
+        }
+#pragma unroll
+        for (int o = 16; o > 0; o >>= 1) cnt += __shfl_xor_sync(B2R_FULL_MASK, cnt, o);
+        if (lane == 0 && cnt != 0) rank[b] -= cnt;
+    }
+}
+
 }  // namespace b2r
 
 using namespace b2r;
+
+// s0 and the unmasked ranks: k_target_score, then k_rank_all over the whole catalogue
+static int rank_all_unmasked(const float* Q, int ldq, const float* I, const int64_t* target, int B, int64_t n_items, int d,
+                             float* s0, int64_t* rank, int32_t* err_flag, cudaStream_t s) {
+    k_target_score<<<(B + kRT - 1) / kRT, kRT, 0, s>>>(Q, ldq, I, target, B, n_items, d, s0, rank, err_flag);
+    B2R_LAUNCH_OK("k_target_score");
+    const int64_t tiles_i = (n_items + kTI - 1) / kTI;
+    B2R_REQUIRE(tiles_i <= 0x7fffffff && (B + kTQ - 1) / kTQ <= 65535, B2R_E_UNSUPPORTED, "b2r_rank_all_items: grid");
+    dim3 grid((unsigned)tiles_i, (unsigned)((B + kTQ - 1) / kTQ));
+    k_rank_all<<<grid, kAT, 0, s>>>(Q, ldq, I, s0, B, n_items, d, reinterpret_cast<unsigned long long*>(rank));
+    B2R_LAUNCH_OK("k_rank_all");
+    return 0;
+}
 
 extern "C" int b2r_gt_rank(const float* pred, int64_t N, int64_t C, int64_t ld, int64_t* rank, b2r_stream_t stream) {
     B2R_REQUIRE(pred && rank, B2R_E_BADARG, "b2r_gt_rank: null pointer");
@@ -173,13 +228,8 @@ extern "C" int b2r_rank_all_items(const float* Q, int ldq, const float* I, const
     B2R_REQUIRE(n_mask == 0 || (mask_row && mask_item), B2R_E_BADARG, "b2r_rank_all_items: mask arrays missing");
     if (B == 0) return 0;
     cudaStream_t s = as_stream(stream);
-    k_target_score<<<(B + kRT - 1) / kRT, kRT, 0, s>>>(Q, ldq, I, target, B, n_items, d, s0, rank, err_flag);
-    B2R_LAUNCH_OK("k_target_score");
-    const int64_t tiles_i = (n_items + kTI - 1) / kTI;
-    B2R_REQUIRE(tiles_i <= 0x7fffffff && (B + kTQ - 1) / kTQ <= 65535, B2R_E_UNSUPPORTED, "b2r_rank_all_items: grid");
-    dim3 grid((unsigned)tiles_i, (unsigned)((B + kTQ - 1) / kTQ));
-    k_rank_all<<<grid, kAT, 0, s>>>(Q, ldq, I, s0, B, n_items, d, reinterpret_cast<unsigned long long*>(rank));
-    B2R_LAUNCH_OK("k_rank_all");
+    const int rc = rank_all_unmasked(Q, ldq, I, target, B, n_items, d, s0, rank, err_flag, s);
+    if (rc != 0) return rc;
     if (n_mask > 0) {
         int64_t g = (n_mask + kRT - 1) / kRT;
         const int64_t cap = (int64_t)sm_count() * 16;
@@ -188,5 +238,28 @@ extern "C" int b2r_rank_all_items(const float* Q, int ldq, const float* I, const
                                              reinterpret_cast<unsigned long long*>(rank), err_flag);
         B2R_LAUNCH_OK("k_rank_unmask");
     }
+    return 0;
+}
+
+extern "C" int b2r_rank_all_items_clicked(const float* Q, int ldq, const float* I, int64_t n_items, int d,
+                                          const int64_t* target, const int64_t* users, int B, const int64_t* clicked_ptr,
+                                          const int64_t* clicked_items, int64_t n_users, float* s0, int64_t* rank,
+                                          int32_t* err_flag, b2r_stream_t stream) {
+    B2R_REQUIRE(Q && I && target && users && clicked_ptr && clicked_items && s0 && rank, B2R_E_BADARG,
+                "b2r_rank_all_items_clicked: null pointer");
+    B2R_REQUIRE(B >= 0 && n_items >= 1 && d >= 1 && ldq >= d && n_users >= 1, B2R_E_BADARG,
+                "b2r_rank_all_items_clicked: bad shape");
+    B2R_REQUIRE(d % 4 == 0 && aligned16(I), B2R_E_UNSUPPORTED, "b2r_rank_all_items_clicked: d=%d must be a multiple of 4",
+                d);
+    if (B == 0) return 0;
+    cudaStream_t s = as_stream(stream);
+    const int rc = rank_all_unmasked(Q, ldq, I, target, B, n_items, d, s0, rank, err_flag, s);
+    if (rc != 0) return rc;
+    int64_t g = (B + kRT / 32 - 1) / (kRT / 32);
+    const int64_t cap = (int64_t)sm_count() * 16;
+    if (g > cap) g = cap;
+    k_rank_unmask_clicked<<<(int)g, kRT, 0, s>>>(Q, ldq, I, s0, users, clicked_ptr, clicked_items, n_users, B, n_items, d,
+                                                 rank, err_flag);
+    B2R_LAUNCH_OK("k_rank_unmask_clicked");
     return 0;
 }

@@ -274,6 +274,32 @@ class ClickedSets:
         self.items = torch.from_numpy(items).to(device)
 
 
+def rank_all_items_clicked(q: torch.Tensor, table: torch.Tensor, target: torch.Tensor, users: torch.Tensor,
+                           clicked: ClickedSets) -> torch.Tensor:
+    """rank_all_items with the masked pairs taken from the clicked-item CSR: row b excludes every item of
+    train_clicked_set[users[b]] | residual_clicked_set[users[b]] (BaseRunner.py:244-251).  Same ranks as
+    rank_all_items given those pairs as COO lists; a user outside [0, n_users) makes check_ids raise IndexError."""
+    if q.dim() != 2 or table.dim() != 2 or q.shape[1] != table.shape[1] or target.numel() != q.shape[0] \
+            or users.numel() != q.shape[0]:
+        raise ValueError("rank_all_items_clicked: q [B, d], table [n_items, d], target [B], users [B]")
+    if clicked.ptr.numel() != clicked.n_users + 1:
+        raise ValueError(f"rank_all_items_clicked: the clicked sets cover {clicked.ptr.numel() - 1} users, "
+                         f"n_users says {clicked.n_users}")
+    _need_cuda(q, table, target, users, clicked.ptr, clicked.items)
+    q, table = _f32c(q, "q"), _f32c(table, "table")
+    target, users = _i64c(target.reshape(-1), "target"), _i64c(users.reshape(-1), "users")
+    B, d = q.shape
+    rank = torch.empty(B, dtype=torch.int64, device=q.device)
+    if B == 0:
+        return rank
+    s0 = torch.empty(B, dtype=torch.float32, device=q.device)
+    _lib.check(_lib.load().b2r_rank_all_items_clicked(_p(q), d, _p(table), table.shape[0], d, _p(target), _p(users), B,
+                                                      _p(clicked.ptr), _p(clicked.items), clicked.n_users, _p(s0),
+                                                      _p(rank), _p(err_flag(q.device)), _stream()),
+               "b2r_rank_all_items_clicked")
+    return rank
+
+
 def _topk_k(k: int) -> int:
     k = int(k)
     if not 1 <= k <= 1024:

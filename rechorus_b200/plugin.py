@@ -132,21 +132,31 @@ class _KernelModelMixin:
     def query_rows(self, feed_dict: dict):
         return None
 
-    def eval_ranks(self, feed_dict: dict, mask_row=None, mask_item=None) -> torch.Tensor:
+    def eval_ranks(self, feed_dict: dict, mask_row=None, mask_item=None, clicked=None) -> torch.Tensor:
         """int64 [B] ranks of the ground-truth item (helpers/BaseRunner.py:63) for one evaluation batch, computed
         on the device.  Under the test_all protocol (candidates = [target] + arange(1, n_items),
         BaseModel.py:194-198) a dot-product model is ranked without materialising the [B, n_items] scores;
-        (mask_row, mask_item) are the (batch row, item id) pairs BaseRunner.py:244-251 would set to -inf."""
+        (mask_row, mask_item) are the (batch row, item id) pairs BaseRunner.py:244-251 would set to -inf.
+        ``clicked`` (ops.ClickedSets, test_all only) names those pairs instead as the clicked items of each row's user;
+        a dot-product model then needs only column 0 of feed_dict["item_id"]."""
         with torch.no_grad():
             opt = self.__dict__.get("_b2r_optimizer")
             if getattr(opt, "exact_dense", False) and not self.training:
                 opt.flush()                     # exact dense-Adam mode: ranks must see rows advanced through skipped steps
             item_id = feed_dict["item_id"]
-            qr = self.query_rows(feed_dict) if getattr(self, "test_all", 0) else None
+            test_all = bool(getattr(self, "test_all", 0))
+            if clicked is not None and test_all and self.has_query_rows():
+                q, table = self.query_rows(feed_dict)
+                return ops.rank_all_items_clicked(q, table, item_id[:, 0], feed_dict["user_id"], clicked)
+            qr = self.query_rows(feed_dict) if test_all else None
             if qr is not None and item_id.shape[1] == self.item_num:
                 q, table = qr
                 return ops.rank_all_items(q, table, item_id[:, 0], mask_row, mask_item)
+            if clicked is not None and test_all and item_id.shape[1] != self.item_num:
+                raise ValueError(f"test_all candidate lists have {self.item_num} columns, got {item_id.shape[1]}")
             pred = self.forward(feed_dict)["prediction"]
+            if clicked is not None and test_all:
+                pred = ops.mask_clicked(pred.contiguous(), feed_dict["user_id"], clicked)
             if mask_row is not None and mask_row.numel() > 0:
                 pred = pred.clone()
                 pred[mask_row, mask_item] = float("-inf")

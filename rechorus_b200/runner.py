@@ -46,6 +46,96 @@ def _poll_ids(model) -> None:
         ops.check_ids(dev if dev.index is not None else None)
 
 
+def eval_history_widths(lengths, B: int) -> List[int]:
+    """The history width of each evaluation batch of B consecutive rows: the longest history in it, the width
+    collate_batch's pad_sequence (or np.array, when all are equal) gives (BaseModel.py:135-152).  lengths: the rows'
+    min(position, history_max) (the whole position when history_max <= 0)."""
+    lengths = np.asarray(lengths, dtype=np.int64)
+    if lengths.size == 0:
+        return []
+    return [int(w) for w in np.maximum.reduceat(lengths, np.arange(0, lengths.size, int(B)))]
+
+
+def history_view(flat: torch.Tensor, Bn: int, width: int) -> torch.Tensor:
+    """A contiguous [Bn, width] batch of histories at the start of one preallocated flat buffer"""
+    return flat[:Bn * width].view(Bn, width)
+
+
+def _eval_state(dataset, B: int) -> dict:
+    """The device inputs of one evaluation phase, uploaded when a device route first evaluates it and cached on the
+    dataset (as fit_on_device caches its state): user / target columns, the fixed neg_items (unless test_all), the
+    clicked-item CSR (test_all), the history CSR (sequential models), and batch buffers for eval_batch_size B."""
+    model = dataset.model
+    st = dataset.__dict__.get("_b2r_eval")
+    dev = model.device
+    corpus, data = dataset.corpus, dataset.data
+    test_all = bool(model.test_all)
+    if st is None:
+        st = {"users": torch.as_tensor(np.asarray(data["user_id"], dtype=np.int64)).to(dev),
+              "targets": torch.as_tensor(np.asarray(data["item_id"], dtype=np.int64)).to(dev), "B": None}
+        if test_all:
+            st["clicked"] = ops.ClickedSets(corpus.train_clicked_set, corpus.residual_clicked_set, corpus.n_users, dev)
+        if hasattr(model, "history_max"):
+            st["his"] = ops.DeviceHistory(corpus.user_his, corpus.n_users, data["user_id"], data["position"],
+                                          model.history_max, dev)
+            pos = np.asarray(data["position"], dtype=np.int64)
+            H = int(model.history_max)
+            st["lens"] = np.minimum(pos, H) if H > 0 else pos    # BaseModel.py:240-242's slice lengths
+        dataset.__dict__["_b2r_eval"] = st
+    N = st["users"].numel()
+    if not test_all and st.get("neg_src") is not data["neg_items"]:
+        st["neg"] = torch.as_tensor(np.asarray(data["neg_items"], dtype=np.int64).reshape(N, -1)).to(dev)
+        st["neg_src"] = data["neg_items"]
+        st["B"] = None
+    if st["B"] != B:
+        bufs = {"user_id": torch.empty(B, dtype=torch.int64, device=dev)}
+        if not test_all:
+            bufs["item_id"] = torch.empty((B, st["neg"].shape[1] + 1), dtype=torch.int64, device=dev)
+        elif not model.has_query_rows():                  # [target | arange(1, n_items)], column 0 per batch
+            bufs["item_id"] = torch.arange(corpus.n_items, dtype=torch.int64, device=dev).repeat(B, 1)
+        if "his" in st:
+            # pad_sequence pads to the batch maximum: each batch's [Bn, Lb] is a contiguous view of one buffer
+            bufs["history_items"] = torch.empty(B * st["his"].width, dtype=torch.int64, device=dev)
+            bufs["lengths"] = torch.empty(B, dtype=torch.int64, device=dev)
+            st["widths"] = eval_history_widths(st["lens"], B)
+        st["bufs"], st["B"] = bufs, B
+    return st
+
+
+def device_eval_batches(dataset, B: int):
+    """Yields (feed dict, clicked sets or None) for the batches of B rows of an evaluation phase (a model's Dataset), in
+    dataset order, built on the device with the same values collate_batch gives (BaseModel.py:135-152,192-203,236-245):
+    b2r_collate_general for the 1 + K candidates, the targets alone for a dot-product model under test_all, a
+    [target | arange(1, n_items)] matrix for other models under test_all, and for sequential models the histories
+    right-padded to the batch's longest one (b2r_collate_history).  Consecutive batches share the buffers: a batch
+    must be consumed (its work enqueued on the current stream) before the next one is requested."""
+    model = dataset.model
+    B = int(B)
+    st = _eval_state(dataset, B)
+    bufs, his, clicked = st["bufs"], st.get("his"), st.get("clicked")
+    users, targets = st["users"], st["targets"]
+    N, test_all = users.numel(), bool(model.test_all)
+    for bi, start in enumerate(range(0, N, B)):
+        Bn = min(B, N - start)
+        feed = {"batch_size": Bn, "phase": dataset.phase}
+        if not test_all:
+            ops.collate_general(users, targets, st["neg"], None, start, Bn, bufs["user_id"], bufs["item_id"])
+            feed["user_id"], feed["item_id"] = bufs["user_id"][:Bn], bufs["item_id"][:Bn]
+        else:
+            feed["user_id"] = users[start:start + Bn]
+            tgt = targets[start:start + Bn].view(-1, 1)
+            if "item_id" in bufs:
+                bufs["item_id"][:Bn, :1].copy_(tgt)
+                feed["item_id"] = bufs["item_id"][:Bn]
+            else:
+                feed["item_id"] = tgt
+        if his is not None:
+            hb = history_view(bufs["history_items"], Bn, st["widths"][bi])
+            his.collate(users, None, start, Bn, hb, bufs["lengths"])
+            feed["history_items"], feed["lengths"] = hb, bufs["lengths"][:Bn]
+        yield feed, clicked
+
+
 class BaseRunner:
     @staticmethod
     def parse_runner_args(parser):
@@ -434,33 +524,22 @@ class BaseRunner:
         return self.evaluate_method(self.predict(dataset), topks, metrics)
 
     def evaluate_on_device(self, dataset, topks: list, metrics: list) -> Dict[str, float]:
-        """helpers/BaseRunner.py:216-252 with the predictions never leaving the GPU: per batch the model returns
-        the integer ranks of the ground truth (``eval_ranks``), a rank histogram is accumulated on the device and
-        HR@k / NDCG@k are read off it -- (max k + 2) integers cross PCIe per evaluation instead of N x C floats."""
+        """helpers/BaseRunner.py:216-252 with neither the inputs nor the predictions on the host: the batches come from
+        ``device_eval_batches`` (no DataLoader, no feed dicts), per batch the model returns the integer ranks of the
+        ground truth (``eval_ranks``; under test_all masked from the clicked-item CSR), a rank histogram is accumulated
+        on the device and HR@k / NDCG@k are read off it -- (max k + 2) integers cross PCIe per evaluation, and the
+        histogram read and the id poll are the only synchronisations."""
         model = dataset.model
         model.eval()
         kmax = max(int(k) for k in topks)
-        hist, n_rows = None, 0
-        dl = DataLoader(dataset, batch_size=self.eval_batch_size, shuffle=False, num_workers=self.num_workers,
-                        collate_fn=dataset.collate_batch, pin_memory=bool(self.pin_memory))
-        start = 0
-        for batch in dl:
-            bs = batch["batch_size"]
-            mask_row = mask_item = None
-            if model.test_all:
-                rows, cols = [], []
-                for i, u in enumerate(dataset.data["user_id"][start:start + bs]):
-                    clicked = list(dataset.corpus.train_clicked_set[u] | dataset.corpus.residual_clicked_set[u])
-                    rows.extend([i] * len(clicked))
-                    cols.extend(clicked)
-                mask_row = torch.tensor(rows, dtype=torch.int64, device=model.device)
-                mask_item = torch.tensor(cols, dtype=torch.int64, device=model.device)
-            batch = batch_to_device(batch, model.device)
-            ranks = model.eval_ranks(batch, mask_row, mask_item)
-            h = ops.rank_histogram(ranks, kmax)
-            hist = h if hist is None else hist + h
-            n_rows += bs
-            start += bs
+        # the host route's DataLoader iterator draws one int64 seed from the global CPU generator: draw it here too, so the
+        # training epochs that follow an evaluation shuffle their rows as the reference's run does
+        torch.empty((), dtype=torch.int64).random_()
+        hist = torch.zeros(kmax + 2, dtype=torch.int64, device=model.device)
+        n_rows = 0
+        for feed, clicked in device_eval_batches(dataset, self.eval_batch_size):
+            hist += ops.rank_histogram(model.eval_ranks(feed, clicked=clicked), kmax)
+            n_rows += feed["batch_size"]
         _poll_ids(model)
         return ops.metrics_from_histogram(hist, n_rows, topks, metrics)
 
@@ -489,53 +568,20 @@ class BaseRunner:
     def recommend(self, dataset, k: int = 100):
         """The top-k' recommendation list of every row of an evaluation phase (main.py:117-132's TopK branch) computed on
         the device: (users as dataset.data["user_id"] holds them, item ids int64 [N, k'], scores float32 [N, k']) as host
-        arrays, rows in dataset order.  Batches of eval_batch_size rows are built on the device, not by the DataLoader:
-        b2r_collate_general over the phase's fixed neg_items (uploaded once), the history slice of ops.DeviceHistory for
-        sequential models, and under test_all either nothing beyond the targets (dot-product models: ops.topk_all_items
-        scores the catalogue) or a [target | arange(1, n_items)] matrix (NeuMF) masked with ops.mask_clicked."""
+        arrays, rows in dataset order.  The batches are evaluate_on_device's (``device_eval_batches``); under test_all a
+        dot-product model scores the catalogue itself (ops.topk_all_items) and NeuMF's [target | arange(1, n_items)]
+        predictions are masked with ops.mask_clicked."""
         model = dataset.model
         model.eval()
-        dev = model.device
-        corpus, data = dataset.corpus, dataset.data
-        N, B = len(dataset), int(self.eval_batch_size)
-        users = torch.as_tensor(np.asarray(data["user_id"], dtype=np.int64)).to(dev)
-        targets = torch.as_tensor(np.asarray(data["item_id"], dtype=np.int64)).to(dev)
-        test_all = bool(model.test_all)
-        clicked = (ops.ClickedSets(corpus.train_clicked_set, corpus.residual_clicked_set, corpus.n_users, dev)
-                   if test_all else None)
-        his = None
-        if hasattr(model, "history_max"):
-            his = ops.DeviceHistory(corpus.user_his, corpus.n_users, data["user_id"], data["position"], model.history_max,
-                                    dev)
-            hist_buf = torch.empty((B, his.width), dtype=torch.int64, device=dev)
-            len_buf = torch.empty(B, dtype=torch.int64, device=dev)
-        if not test_all:
-            neg = torch.as_tensor(np.asarray(data["neg_items"], dtype=np.int64).reshape(N, -1)).to(dev)
-            uid_buf = torch.empty(B, dtype=torch.int64, device=dev)
-            iid_buf = torch.empty((B, neg.shape[1] + 1), dtype=torch.int64, device=dev)
-        elif not model.has_query_rows():
-            arange = torch.arange(1, corpus.n_items, dtype=torch.int64, device=dev)
         out_items, out_scores = [], []
-        for start in range(0, N, B):
-            Bn = min(B, N - start)
-            feed = {"batch_size": Bn, "phase": dataset.phase}
-            if test_all:
-                tgt = targets[start:start + Bn].view(-1, 1)
-                feed["user_id"] = users[start:start + Bn]
-                feed["item_id"] = tgt if model.has_query_rows() else torch.cat([tgt, arange.expand(Bn, -1)], dim=1)
-            else:
-                ops.collate_general(users, targets, neg, None, start, Bn, uid_buf, iid_buf)
-                feed["user_id"], feed["item_id"] = uid_buf[:Bn], iid_buf[:Bn]
-            if his is not None:
-                his.collate(users, None, start, Bn, hist_buf, len_buf)
-                feed["history_items"], feed["lengths"] = hist_buf[:Bn], len_buf[:Bn]
+        for feed, clicked in device_eval_batches(dataset, self.eval_batch_size):
             items, scores = model.recommend(feed, k, clicked)
             out_items.append(items)
             out_scores.append(scores)
         _poll_ids(model)
         if not out_items:
-            return list(data["user_id"]), np.zeros((0, 0), np.int64), np.zeros((0, 0), np.float32)
-        return (list(data["user_id"]), torch.cat(out_items).cpu().numpy(), torch.cat(out_scores).cpu().numpy())
+            return list(dataset.data["user_id"]), np.zeros((0, 0), np.int64), np.zeros((0, 0), np.float32)
+        return (list(dataset.data["user_id"]), torch.cat(out_items).cpu().numpy(), torch.cat(out_scores).cpu().numpy())
 
     def save_rec_results(self, dataset, result_path: str, topk: int = 100, sep: str = "\t") -> None:
         """The TopK branch of main.py:117-132 (save_rec_results) with the lists from ``recommend``: same columns and
