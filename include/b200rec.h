@@ -384,9 +384,21 @@ B2R_API int b2r_select_last(const float* y, const int64_t* hist, const int64_t* 
                     int d, b2r_stream_t stream);
 B2R_API int b2r_select_last_bwd(const float* dh, const int64_t* hist, const int64_t* lengths, float* dy, int B, int L,
                         int d, b2r_stream_t stream);
+/* small_table_grad keeps G = 256 / d copies of the table in shared memory (G = 1 when d does not divide 256) and
+ * returns B2R_E_UNSUPPORTED when they exceed 200 KB, e.g. more than 200 rows at d in {32, 64, 128}; callers then use the
+ * plan route (b2r_plan_* / b2r_direct_plan_*), which has no size limit. */
 B2R_API size_t b2r_small_table_grad_workspace_bytes(int64_t n, int n_rows, int d);
 B2R_API int b2r_small_table_grad(const float* src, int ld, const int64_t* ids, int64_t n, int n_rows, int d,
                          float* dense_out, void* ws, size_t ws_bytes, b2r_stream_t stream);
+
+/* Training envelope of SASRec: 0 when every kernel of a training step (forward and backward) accepts batches of width
+ * 1..L at embedding width d with H heads, else B2R_E_UNSUPPORTED with b2r_last_error() naming the refusing kernel and its
+ * limit.  full_blocks = the blocks that run full causal attention; flags: B2R_SEQ_LAST_QUERY when the last block runs for
+ * the one query per sequence (b2r_attention_last_*), B2R_SEQ_ATTN_V1 when full attention always takes the shared-memory
+ * kernels (b2r_attention_*_live) instead of trying b2r_attention_*_rt first.  Host only: no device call is made. */
+#define B2R_SEQ_LAST_QUERY 1
+#define B2R_SEQ_ATTN_V1 2
+B2R_API int b2r_seq_train_check(int L, int d, int H, int full_blocks, int flags);
 
 /* out[r,k] = a[r,k] * w[k]   and   out[k] = sum_r a[r,k] * b[r,k]   (the GMF half of NeuMF's final Linear,
  * models/general/NeuMF.py:68,74-75, and its weight gradient) */

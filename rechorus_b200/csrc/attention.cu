@@ -11,6 +11,7 @@
 // (layers.py:60), a scalar shift that cancels; the kernels subtract the row max (same function, no
 // cross-row underflow).  Fully masked rows cannot occur under the causal mask (key j = query i is allowed).
 #include "common.cuh"
+#include "seq_limits.cuh"
 
 namespace b2r {
 
@@ -369,11 +370,6 @@ extern "C" int b2r_embed_history(const float* I, int64_t n_items, const float* P
     return 0;
 }
 
-static size_t attn_fwd_smem(int L, int d, int H) { return ((size_t)3 * L * (d + 1) + (size_t)8 * H * L) * sizeof(float); }
-static size_t attn_bwd_smem(int L, int d, int H) {
-    return ((size_t)4 * L * (d + 1) + (size_t)H * L * (L + 1)) * sizeof(float);
-}
-
 extern "C" int b2r_attention_fwd_live(const float* q, const float* k, const float* v, int ld, const int64_t* live, float* ctx,
                                       int B, int L, int d, int H, b2r_stream_t stream) {
     B2R_REQUIRE(q && k && v && ctx, B2R_E_BADARG, "b2r_attention_fwd: null pointer");
@@ -381,7 +377,7 @@ extern "C" int b2r_attention_fwd_live(const float* q, const float* k, const floa
                 "b2r_attention_fwd: bad shape B=%d L=%d d=%d H=%d ld=%d", B, L, d, H, ld);
     if (B == 0) return 0;
     const size_t smem = attn_fwd_smem(L, d, H);
-    B2R_REQUIRE(smem <= 227 * 1024, B2R_E_UNSUPPORTED, "b2r_attention_fwd: L=%d d=%d needs %zu B of shared memory", L, d,
+    B2R_REQUIRE(smem <= kAttnSmemMax, B2R_E_UNSUPPORTED, "b2r_attention_fwd: L=%d d=%d needs %zu B of shared memory", L, d,
                 smem);
     B2R_CUDA_OK(cudaFuncSetAttribute(k_attention_fwd, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     k_attention_fwd<<<B, 256, smem, as_stream(stream)>>>(q, k, v, ld, ctx, L, d, H, 1.f / sqrtf((float)(d / H)), live);
@@ -398,11 +394,11 @@ extern "C" int b2r_attention_bwd_live(const float* q, const float* k, const floa
                                       const float* dctx, float* dq, float* dk, float* dv, int ldg, int B, int L, int d, int H,
                                       b2r_stream_t stream) {
     B2R_REQUIRE(q && k && v && dctx && dq && dk && dv, B2R_E_BADARG, "b2r_attention_bwd: null pointer");
-    B2R_REQUIRE(B >= 0 && L > 0 && L <= 128 && d > 0 && H > 0 && d % H == 0 && ld >= d && ldg >= d, B2R_E_BADARG,
+    B2R_REQUIRE(B >= 0 && L > 0 && L <= kAttnBwdMaxL && d > 0 && H > 0 && d % H == 0 && ld >= d && ldg >= d, B2R_E_BADARG,
                 "b2r_attention_bwd: bad shape B=%d L=%d d=%d H=%d", B, L, d, H);
     if (B == 0) return 0;
     const size_t smem = attn_bwd_smem(L, d, H);
-    B2R_REQUIRE(smem <= 227 * 1024, B2R_E_UNSUPPORTED, "b2r_attention_bwd: L=%d d=%d H=%d needs %zu B of shared memory",
+    B2R_REQUIRE(smem <= kAttnSmemMax, B2R_E_UNSUPPORTED, "b2r_attention_bwd: L=%d d=%d H=%d needs %zu B of shared memory",
                 L, d, H, smem);
     B2R_CUDA_OK(cudaFuncSetAttribute(k_attention_bwd, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     k_attention_bwd<<<B, 256, smem, as_stream(stream)>>>(q, k, v, ld, dctx, dq, dk, dv, ldg, L, d, H,

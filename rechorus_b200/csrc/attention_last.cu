@@ -1,4 +1,5 @@
-// attention_last.cu -- groundwork for the next round (opt-in via B2R_SASREC_LASTQ=1, not yet run on a GPU).
+// attention_last.cu -- SASRec's last block for one query per sequence (the default route; B2R_SASREC_LASTQ=0 runs the
+// full block instead).  Batch widths up to kALMaxL = 256 (seq_limits.cuh).
 //
 // SASRec scores candidates against ONE vector per sequence: the encoder state at position len-1 of the LAST block
 // (models/sequential/SASRec.py:74-81).  Every other position of the last block's output is dead, so for that block
@@ -11,11 +12,11 @@
 //   k_attention_last_bwd  same decomposition: dV = p (x) dctx, dS = p * (dP - <p, dP>), dq = scale * dS K,
 //                         dK = scale * dS (x) q; rows beyond t* get exact zeros.  Every element has one writer.
 #include "common.cuh"
+#include "seq_limits.cuh"
 
 namespace b2r {
 
 constexpr int kALWarps = 8;
-constexpr int kALMaxL = 256;
 
 __global__ void __launch_bounds__(kALWarps * 32)
 k_attention_last_fwd(const float* __restrict__ q, const float* __restrict__ k, const float* __restrict__ v, int ld,

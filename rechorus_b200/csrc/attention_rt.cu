@@ -16,6 +16,7 @@
 // t >= live[b] are dead (nothing downstream reads them; their upstream gradient is zero): skipped, outputs written as
 // zeros -- same contract as attention.cu.
 #include "common.cuh"
+#include "seq_limits.cuh"
 
 namespace b2r {
 
@@ -225,15 +226,6 @@ k_attention_bwd_rt(const float* __restrict__ q, const float* __restrict__ k, con
     stage_out(dv, row0, ldg, vs, S, Lq, L, d4);
 }
 
-static bool rt_shape_ok(int L, int d, int H, int ld) {
-    if (H <= 0 || d % H != 0) return false;
-    const int dk = d / H;
-    return (dk == 8 || dk == 16 || dk == 32) && L <= 128 && d % 4 == 0 && ld % 4 == 0;
-}
-
-static size_t rt_fwd_smem(int L, int d) { return (size_t)3 * L * (d + 4) * sizeof(float); }
-static size_t rt_bwd_smem(int L, int d, int H) { return ((size_t)5 * L * (d + 4) + (size_t)2 * L * H) * sizeof(float); }
-
 }  // namespace b2r
 
 using namespace b2r;
@@ -250,7 +242,7 @@ extern "C" int b2r_attention_fwd_rt(const float* q, const float* k, const float*
     B2R_REQUIRE(q && k && v && ctx && lse, B2R_E_BADARG, "b2r_attention_fwd_rt: null pointer");
     B2R_REQUIRE(B >= 0 && L > 0 && d > 0 && ld >= d, B2R_E_BADARG, "b2r_attention_fwd_rt: bad shape B=%d L=%d d=%d ld=%d", B, L, d, ld);
     const size_t smem = rt_fwd_smem(L, d);
-    if (!rt_shape_ok(L, d, H, ld) || smem > 227 * 1024 || !aligned16(q) || !aligned16(k) || !aligned16(v) || !aligned16(ctx))
+    if (!rt_shape_ok(L, d, H, ld) || smem > kAttnSmemMax || !aligned16(q) || !aligned16(k) || !aligned16(v) || !aligned16(ctx))
         return b2r::set_error(B2R_E_UNSUPPORTED, "b2r_attention_fwd_rt: L=%d d=%d H=%d ld=%d not covered (use b2r_attention_fwd_live)", L, d, H, ld);
     if (B == 0) return 0;
     const float scale2 = kLog2e / sqrtf((float)(d / H));
@@ -268,7 +260,7 @@ extern "C" int b2r_attention_bwd_rt(const float* q, const float* k, const float*
     B2R_REQUIRE(q && k && v && ctx && lse && dctx && dq && dk && dv, B2R_E_BADARG, "b2r_attention_bwd_rt: null pointer");
     B2R_REQUIRE(B >= 0 && L > 0 && d > 0 && ld >= d && ldg >= d, B2R_E_BADARG, "b2r_attention_bwd_rt: bad shape B=%d L=%d d=%d", B, L, d);
     const size_t smem = rt_bwd_smem(L, d, H);
-    if (!rt_shape_ok(L, d, H, ld) || ldg % 4 != 0 || smem > 227 * 1024 || !aligned16(q) || !aligned16(k) || !aligned16(v) ||
+    if (!rt_shape_ok(L, d, H, ld) || ldg % 4 != 0 || smem > kAttnSmemMax || !aligned16(q) || !aligned16(k) || !aligned16(v) ||
         !aligned16(ctx) || !aligned16(dctx) || !aligned16(dq) || !aligned16(dk) || !aligned16(dv))
         return b2r::set_error(B2R_E_UNSUPPORTED, "b2r_attention_bwd_rt: L=%d d=%d H=%d not covered (use b2r_attention_bwd_live)", L, d, H);
     if (B == 0) return 0;

@@ -6,6 +6,7 @@
 // fp32 FMA on the CUDA cores keeps the 1e-5 parity bar of the north star; linear_tc.cu and linear_dw_tc.cu are the
 // tensor-core (3xTF32 / 4xTF32 wgmma) versions for long batches.
 #include "common.cuh"
+#include "seq_limits.cuh"
 #include "dropout.cuh"
 
 namespace b2r {
@@ -434,7 +435,8 @@ static int add_layernorm_fwd(const float* x, const float* res, const float* gamm
                              float* mean, float* rstd, int64_t rows, int d, float eps, const DropK* drop, cudaStream_t s) {
     B2R_REQUIRE(x && res && gamma && beta && y && mean && rstd, B2R_E_BADARG, "b2r_add_layernorm_fwd: null pointer");
     B2R_REQUIRE(rows >= 0 && d > 0, B2R_E_BADARG, "b2r_add_layernorm_fwd: bad shape");
-    B2R_REQUIRE(drop == nullptr || d <= 256, B2R_E_UNSUPPORTED, "b2r_add_layernorm_fwd_dropout: need d <= 256 (d=%d)", d);
+    B2R_REQUIRE(drop == nullptr || d <= kLNMaxD, B2R_E_UNSUPPORTED, "b2r_add_layernorm_fwd_dropout: need d <= %d (d=%d)",
+                kLNMaxD, d);
     if (rows == 0) return 0;
     int64_t need = (rows + 7) / 8;
     const int64_t cap = (int64_t)sm_count() * 16;
@@ -468,7 +470,8 @@ static int add_layernorm_bwd(const float* dy, const float* x, const float* res, 
                              void* ws, size_t ws_bytes, const DropK* drop, cudaStream_t s) {
     B2R_REQUIRE(dy && x && res && gamma && mean && rstd && dz && dgamma && dbeta && ws && (drop == nullptr || dx),
                 B2R_E_BADARG, "b2r_add_layernorm_bwd: null pointer");
-    B2R_REQUIRE(rows > 0 && d > 0 && d <= 256, B2R_E_UNSUPPORTED, "b2r_add_layernorm_bwd: need 0 < d <= 256 (d=%d)", d);
+    B2R_REQUIRE(rows > 0 && d > 0 && d <= kLNMaxD, B2R_E_UNSUPPORTED, "b2r_add_layernorm_bwd: need 0 < d <= %d (d=%d)",
+                kLNMaxD, d);
     B2R_REQUIRE(ws_bytes >= b2r_add_layernorm_bwd_workspace_bytes(rows, d), B2R_E_WORKSPACE,
                 "b2r_add_layernorm_bwd: workspace too small");
     const int ctas = ln_bwd_ctas(rows);

@@ -42,6 +42,7 @@ class Dropout(C.Structure):
 
 
 OPT_SGD, OPT_ADAM, OPT_ADAGRAD = 0, 1, 2
+SEQ_LAST_QUERY, SEQ_ATTN_V1 = 1, 2          # b2r_seq_train_check flags
 PROF_SCORE_FWD, PROF_SCORE_BWDQ, PROF_SEGMENT_I, PROF_SEGMENT_U, PROF_PLAN_I, PROF_LOSS = range(6)
 
 # name -> (restype, argtypes); must list every symbol include/b200rec.h declares (tests/test_abi.py checks)
@@ -147,6 +148,7 @@ SIGNATURES = {
     "b2r_small_table_grad_workspace_bytes": (C.c_size_t, [C.c_int64, C.c_int, C.c_int]),
     "b2r_small_table_grad": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p, C.c_int64, C.c_int, C.c_int, C.c_void_p,
                                        C.c_void_p, C.c_size_t, C.c_void_p]),
+    "b2r_seq_train_check": (C.c_int, [C.c_int, C.c_int, C.c_int, C.c_int, C.c_int]),
     "b2r_colscale": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_int, C.c_void_p]),
     "b2r_gt_rank": (C.c_int, [C.c_void_p, C.c_int64, C.c_int64, C.c_int64, C.c_void_p, C.c_void_p]),
     "b2r_rank_histogram": (C.c_int, [C.c_void_p, C.c_int64, C.c_int, C.c_void_p, C.c_void_p]),

@@ -1317,9 +1317,21 @@ def causal_attention(q, k, v, num_heads, live=None):
     return _CausalAttention.apply(q, k, v, num_heads, live)
 
 
+def seq_train_error(L: int, d: int, H: int, num_layers: int, last_query: bool) -> Optional[str]:
+    """None when a SASRec training step on batches of width up to L runs on the kernels (b2r_seq_train_check, with the
+    attention route this process takes), else the library's reason.  last_query: the last block runs for the one query
+    per sequence (attention_last)."""
+    last_query = bool(last_query) and num_layers > 0
+    flags = (_lib.SEQ_LAST_QUERY if last_query else 0) | (0 if _ATTN_RT else _lib.SEQ_ATTN_V1)
+    L_ = _lib.load()
+    rc = L_.b2r_seq_train_check(int(L), int(d), int(H), int(num_layers) - int(last_query), flags)
+    return None if rc == 0 else L_.b2r_last_error().decode("utf-8", "replace")
+
+
 class _AttentionLast(torch.autograd.Function):
     """Attention for the one query per sequence that SASRec's last block needs (position len-1): q_last [B, d] against
-    k, v [B, L, d]; identical to row len-1 of _CausalAttention.  Opt-in groundwork (B2R_SASREC_LASTQ=1)."""
+    k, v [B, L, d]; identical to row len-1 of _CausalAttention.  SASRec's last block runs on it by default
+    (B2R_SASREC_LASTQ=0 runs the full block instead); L <= 256."""
 
     @staticmethod
     def forward(ctx, q_last, k, v, lengths, H):
@@ -1384,8 +1396,11 @@ class _EmbedHistory(torch.autograd.Function):
             gP = torch.empty_like(P)
             L = _lib.load()
             ws = _ws(L.b2r_small_table_grad_workspace_bytes(n, P.shape[0], d), dx.device)
-            _lib.check(L.b2r_small_table_grad(_p(dx2), d, _p(pos), n, P.shape[0], d, _p(gP), _p(ws), ws.numel(),
-                                              _stream()), "b2r_small_table_grad")
+            rc = L.b2r_small_table_grad(_p(dx2), d, _p(pos), n, P.shape[0], d, _p(gP), _p(ws), ws.numel(), _stream())
+            if rc == -3:                    # B2R_E_UNSUPPORTED: the table's shared-memory copies do not fit
+                gP = _table_grad(P, pos, Source(src=dx2, n=n))
+            else:
+                _lib.check(rc, "b2r_small_table_grad")
         return gI, gP, None, None
 
 

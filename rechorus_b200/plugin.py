@@ -367,7 +367,13 @@ class SASRecKernels(_KernelModelMixin):
         self.num_heads = args.num_heads
         if self.emb_size % 4 != 0 or self.emb_size % self.num_heads != 0:
             raise ValueError("rechorus_b200 kernels need emb_size % 4 == 0 and emb_size % num_heads == 0")
-        ops.check_dropout_p(self.dropout)                     # the reference's nn.Dropout(dropout) (layers.py:104,110)
+        if self.max_his > 0:
+            # refused here rather than by the first backward (DESIGN.md, a8-a10: the trainable envelope)
+            err = ops.seq_train_error(self.max_his, self.emb_size, self.num_heads, self.num_layers, _SASREC_LASTQ)
+            if err is not None:
+                raise ValueError(f"SASRec cannot train with history_max={self.max_his}, emb_size={self.emb_size}, "
+                                 f"num_heads={self.num_heads}, num_layers={self.num_layers} on these kernels: {err}")
+        ops.check_dropout_p(self.dropout)                    # the reference's nn.Dropout(dropout) (layers.py:104,110)
         self._dropout_init()
         self._base_define_params()
         self.apply(self.init_weights)
