@@ -25,7 +25,7 @@
 extern "C" {
 #endif
 
-#define B2R_VERSION 101          /* major*10000 + minor*100 + patch */
+#define B2R_VERSION 102          /* major*10000 + minor*100 + patch */
 
 #define B2R_E_BADARG   (-1)      /* null pointer, d % 4 != 0, negative size ... */
 #define B2R_E_WORKSPACE (-2)     /* workspace too small */
@@ -177,45 +177,16 @@ B2R_API int b2r_segment_apply(const uint32_t* sorted_key, const uint32_t* sorted
                       float* W, float* m, float* v, const b2r_optim* opt, b2r_stream_t stream);
 
 /* ------------------------------------------------------------------------------------------------
- * Bucketed form of plan + segment for the hot path (modes 1 and 2 only; d in {32, 64, 128}):
- *   b2r_bucket_partition : two passes over the ids partition the (row id, position) pairs into buckets of
- *                          2^shift consecutive table rows (~200 pairs each) with L2 atomics;
- *   b2r_bucket_apply     : one CTA per bucket sorts its pairs by (row, position) in shared memory and applies
- *                          mode 1 (dense[row] += gradient row) or mode 2 (optimizer in place), each row's
- *                          contributions summed in ascending position -> same bits on every run.
- * The workspace must have been initialised once with b2r_bucket_workspace_init (zeroed counters); partition
- * leaves the counters zero again, so the same workspace is reusable step after step.
+ * Bucketed form of plan + segment for the hot path ("direct" plans; modes 1 and 2 only; d in {32, 64, 128}):
+ *   b2r_direct_plan_build : every (row id, position) pair is dropped into the fixed-capacity region of its bucket of
+ *                           2^shift consecutive table rows (~200 pairs each) with one L2 atomic (pairs beyond a
+ *                           region's capacity go to a spill list), then one kernel sorts every bucket by (row, position)
+ *                           in shared memory and lists the row heads;
+ *   b2r_direct_plan_apply : mode 1 (dense[row] += gradient row) or mode 2 (optimizer in place), each row's
+ *                           contributions summed in ascending position -> same bits on every run.
+ * The workspace must be initialised once with b2r_direct_plan_init; build/apply may then alternate.
+ * b2r_direct_plan_workspace_bytes returns 0 for shapes it cannot take (n > 2^30 - 1, n_rows >= 2^32 - 1).
  * ---------------------------------------------------------------------------------------------- */
-B2R_API size_t b2r_bucket_workspace_bytes(int64_t n, int64_t n_rows);
-B2R_API int b2r_bucket_workspace_init(void* ws, size_t ws_bytes, int64_t n, int64_t n_rows, b2r_stream_t stream);
-B2R_API int b2r_bucket_partition(const int64_t* ids, int64_t n, int64_t n_rows, int64_t ignore_id, int64_t ignore_n,
-                         void* ws, size_t ws_bytes, int32_t* err_flag, b2r_stream_t stream);
-B2R_API int b2r_bucket_apply(const void* ws, int64_t n, int64_t n_rows, int d, const b2r_grad_source* s0,
-                     const b2r_grad_source* s1, int mode, float* dense, float* W, float* m, float* v,
-                     const b2r_optim* opt, b2r_stream_t stream);
-
-/* One table's share of an apply launch (same meaning as the b2r_bucket_apply arguments of those names). */
-typedef struct b2r_apply_job {
-    const void* ws;              /* the table's plan: workspace filled by b2r_bucket_partition */
-    int64_t n, n_rows;
-    const b2r_grad_source* s0;
-    const b2r_grad_source* s1;   /* optional second contribution stream (NULL: none) */
-    float* dense;                /* mode 1 */
-    float* W;                    /* mode 2 */
-    float* m;
-    float* v;
-} b2r_apply_job;
-
-/* b2r_bucket_apply for two tables in ONE launch (job b may be NULL): the two updates must be independent -- neither
- * job's sources may alias the other job's W -- e.g. the user and the item table of one BPRMF step, the item gradient
- * reading a saved copy of the user rows.  The small table's update then runs underneath the large one's. */
-B2R_API int b2r_bucket_apply_pair(const b2r_apply_job* a, const b2r_apply_job* b, int d, int mode, const b2r_optim* opt,
-                                  b2r_stream_t stream);
-
-/* "Direct" plans: the same plan as b2r_bucket_partition in two launches instead of four -- every (row, position) pair is
- * dropped into the fixed-capacity region of its row range with one L2 atomic (pairs beyond a region's capacity go to a
- * spill list), then one kernel sorts every bucket and lists the row heads.  b2r_direct_plan_apply == b2r_bucket_apply on
- * such a plan.  The workspace must be initialised once with b2r_direct_plan_init; build/apply may then alternate. */
 B2R_API size_t b2r_direct_plan_workspace_bytes(int64_t n, int64_t n_rows);
 B2R_API int b2r_direct_plan_init(void* ws, size_t ws_bytes, int64_t n, int64_t n_rows, b2r_stream_t stream);
 B2R_API int b2r_direct_plan_build(const int64_t* ids, int64_t n, int64_t n_rows, int64_t ignore_id, int64_t ignore_n,
@@ -439,7 +410,7 @@ B2R_API int b2r_collate_history(const int64_t* users, const int64_t* positions, 
  * table (helpers/BaseRunner.py:110-114,206) would have moved them with a zero data gradient (g = weight_decay * w).
  * last [n_rows] int32 holds the step each row is up to date with.  rows == NULL: all n_rows rows (flush); otherwise n
  * unique row ids.  Every processed row is brought to step `upto` and stamped max(upto, stamp) -- pass stamp = upto + 1
- * when the step-(upto+1) update with b2r_bucket_apply / b2r_segment_apply follows.  opt carries lr, betas, eps,
+ * when the step-(upto+1) update with b2r_direct_plan_apply / b2r_segment_apply follows.  opt carries lr, betas, eps,
  * weight_decay, state_ld (kind must be Adam; bc1/bc2 are not used: every skipped step has its own).
  * ---------------------------------------------------------------------------------------------- */
 B2R_API int b2r_adam_exact_advance(const int64_t* rows, int64_t n, int64_t n_rows, int d, float* W, float* m, float* v,
@@ -532,12 +503,12 @@ B2R_API int b2r_topk_all_items(const float* Q, int ldq, const float* I, int64_t 
                                void* workspace, size_t workspace_bytes, b2r_stream_t stream);
 
 /* ------------------------------------------------------------------------------------------------
- * Fused BPRMF forward + loss + query-side backward: every candidate row is read from HBM once and stays in
- * registers between scoring and the gradient.  Outputs: grad_pred [B,C] (= d loss / d pred, loss = mean of the
- * per-sample losses), row_loss [B] (per-sample -log S), dQ [B,d] (= sum_c g[b,c] I[iid[b,c]]), pred [B,C]
- * optional (NULL to skip).  Returns B2R_E_UNSUPPORTED when no fused variant exists for (d, C) -- callers then
- * use b2r_rowdot_fwd / b2r_bpr_loss / b2r_rowdot_bwd_query.  Replaces BPRMF.py:39-42, BaseModel.py:182-185
- * and their autograd (BaseRunner.py:205) in one kernel.
+ * Fused BPRMF forward + loss + query-side backward in one streaming pass: every candidate row is read from HBM once
+ * and used once (online-softmax recurrence for the gradient).  Outputs: grad_pred [B,C] (= d loss / d pred, loss = mean
+ * of the per-sample losses), row_loss [B] (per-sample -log S), dQ [B,d] (= sum_c g[b,c] I[iid[b,c]]), pred [B,C]
+ * optional (NULL to skip).  Returns B2R_E_UNSUPPORTED outside the kernel's class -- d not in {32, 64, 128}, C > 1024,
+ * n_users, n_items or B*C >= 2^32 - 1 -- callers then use b2r_rowdot_fwd / b2r_bpr_loss / b2r_rowdot_bwd_query.
+ * Replaces BPRMF.py:39-42, BaseModel.py:182-185 and their autograd (BaseRunner.py:205) in one kernel.
  * ---------------------------------------------------------------------------------------------- */
 B2R_API int b2r_bprmf_fused_fwd_bwd(const float* U, const int64_t* uid, int64_t n_users, const float* I,
                             const int64_t* iid, int64_t n_items, float* pred, float* grad_pred, float* row_loss,
@@ -551,7 +522,9 @@ B2R_API int b2r_bprmf_fused_fwd_bwd(const float* U, const int64_t* uid, int64_t 
  * The context owns a side stream on which the index plans (sorts) are built; passing the NEXT batch's ids
  * (next_uid/next_iid, device pointers that must stay unmodified until the next call) lets the sort of step
  * t+1 overlap the HBM-bound kernels of step t, like a data loader's prefetch.  Pass NULLs to disable.
- * The workspace (b2r_bprmf_step_workspace_bytes) is caller-owned and must outlive the context.
+ * The workspace (b2r_bprmf_step_workspace_bytes) is caller-owned and must outlive the context.  Shapes whose index
+ * plans cannot be sized (b2r_direct_plan_workspace_bytes == 0 for the item or the user table) get 0 bytes and
+ * B2R_E_UNSUPPORTED from b2r_bprmf_ctx_create.
  * ---------------------------------------------------------------------------------------------- */
 typedef struct {
     float*  U;  float* I;            /* [n_users, d], [n_items, d]                       */

@@ -1,36 +1,36 @@
 // bprmf_flash.cu -- K1+K2a as ONE streaming pass per sample, no second use of any candidate row.
 //
-// Contract (same as the kernels it replaces, bprmf_fused.cu): gather the user row and the C candidate rows of a
-// sample, score them (models/general/BPRMF.py:39-42), evaluate the BPR loss (models/BaseModel.py:182-185) and its
-// closed-form gradient g (SURVEY.md A.4), and reduce dQ = sum_c g_c * I[id_c] (the mul/sum half of loss.backward(),
-// helpers/BaseRunner.py:205) -- every candidate row read from HBM exactly once.
+// Contract: gather the user row and the C candidate rows of a sample, score them (models/general/BPRMF.py:39-42),
+// evaluate the BPR loss (models/BaseModel.py:182-185) and its closed-form gradient g (SURVEY.md A.4), and reduce
+// dQ = sum_c g_c * I[id_c] (the mul/sum half of loss.backward(), helpers/BaseRunner.py:205) -- every candidate row read
+// from HBM exactly once.
 //
-// Why a new structure: the earlier kernels kept all rows of a sample on chip between their two uses (score, then
-// g * row once the softmax over the sample's negatives is known) and were bound by that hand-over (barriers, cross-group
-// statistics, 22 M warp instructions for 105 MB).  The gradient factorises instead.  With e_c = exp(x_c - M),
-// s_c = sigmoid(p - x_c), Z = sum e_c, A = sum e_c s_c, S = A / Z, dS = -1 / (B S):
+// Why this structure: keeping all rows of a sample on chip between their two uses (score, then g * row once the softmax
+// over the sample's negatives is known) is bound by that hand-over (barriers, cross-group statistics).  The gradient
+// factorises instead.  With e_c = exp(x_c - M), s_c = sigmoid(p - x_c), Z = sum e_c, A = sum e_c s_c, S = A / Z,
+// dS = -1 / (B S):
 //     g_c = dS * (e_c / Z) * ((s_c - S) - s_c (1 - s_c)) = (dS / Z) * e_c * (s_c^2 - S)        (negatives)
 //     dQ  = g_0 * r_0 + (dS / Z) * ( sum_c e_c s_c^2 r_c  -  S * sum_c e_c r_c )
 // so two row-weighted sums (acc1, acc2) and three scalars (Z, A, D = sum e_c s_c (1 - s_c)) can be accumulated while
 // the rows stream through, with the running-max rescaling of an online softmax -- the flash-attention recurrence
 // applied to BPR.  A row is needed for one dot product and two FMAs and is then dead.
 //
-// Decomposition: ONE WARP per sample, no block-level barrier anywhere.  A row is read by LPR = d/(4 VPL) lanes (VPL x 16 B
-// each: VPL = 2 halves the per-row share of the reductions, exponentials and broadcasts against VPL = 1);
+// Decomposition: ONE WARP per sample, no block-level barrier anywhere.  A row is read by LPR = d/4 lanes (16 B each);
 // the warp's 32 / LPR lane groups take alternate negatives.  Rows travel global -> shared memory with cp.async (16 B per
-// lane, nothing held in registers while in flight) through a per-warp ring of ST stages of RCH rows per group, so
-// (ST - 1) * RCH rows per group are always in flight; each lane reads back only the 16 bytes it copied itself.  The
-// sample's ids are fetched first (one coalesced pass) and parked in shared memory as checked 32-bit row indices.  The
-// groups' partial states meet once per sample through shuffles (online-softmax combine, fixed order -> deterministic).
-// All 8 warps x 4 CTAs per SM of a B = 4096 batch are resident at once: a single wave, no tail.
-#include <stdlib.h>
-
+// lane, nothing held in registers while in flight) through a per-warp ring of kFlStages stages of kFlRows rows per group,
+// so (kFlStages - 1) * kFlRows rows per group are always in flight; each lane reads back only the 16 bytes it copied
+// itself.  The sample's ids are fetched first (one coalesced pass) and parked in shared memory as checked 32-bit row
+// indices.  The groups' partial states meet once per sample through shuffles (online-softmax combine, fixed order ->
+// deterministic).  All 8 warps x 4 CTAs per SM of a B = 4096 batch are resident at once: a single wave, no tail.
+// Two float4 per lane execute fewer instructions but spill under the 64-register cap that residency needs, and measured
+// slower (0.152 vs 0.150 ms per config-2 step).
 #include "common.cuh"
-#include "plan_direct.cuh"
 
 namespace b2r {
 
-constexpr int kFlMaxWarps = 8;
+constexpr int kFlWarps = 8;       // samples in flight per CTA; 512 CTAs at B = 4096, 4 per SM, all of its shared memory
+constexpr int kFlRows = 4;        // rows per lane group per chunk
+constexpr int kFlStages = 3;      // ring stages
 
 // sum each of the RCH per-lane values over the LPR lanes of a group with ~RCH + log2(LPR / RCH) shuffles: at every step
 // the lanes split the live values in two halves and exchange the half they give up.  Afterwards lane `sub` holds the
@@ -73,60 +73,39 @@ __device__ __forceinline__ void fl_cp16(void* smem_dst, const void* gsrc, bool v
     asm volatile("cp.async.cg.shared.global [%0], [%1], 16, %2;\n" ::"r"(sa), "l"(gsrc), "r"(nbytes) : "memory");
 }
 
-// D floats per row; VPL float4 per lane per row (LPR = D / (4 VPL) lanes share a row); RCH rows per lane group per chunk;
-// ST ring stages.  Per warp the ring holds ST * RCH * (32 / LPR) rows = ST * RCH * VPL * 512 bytes.
-// PLAN: also drop every (row, position) pair of the batch into the update's index plan (plan_direct.cuh) while the ids
-// pass through -- the step then needs no partition pass of its own.
-// WPC warps (= samples in flight) per CTA: 8 (default; 512 CTAs, 4 per SM, take all of an SM's shared memory) or 7 (586
-// CTAs, leave ~34 KB of shared memory per SM for co-resident plan CTAs of the side stream -- measured slower in the step).
-template <int D, int VPL, int RCH, int ST, bool PLAN, int WPC>
-__global__ void __launch_bounds__(WPC * 32, (ST * RCH * VPL <= 12) ? 4 : 2)
+// D floats per row.  Per warp the ring holds kFlStages * kFlRows * (32 / LPR) rows = kFlStages * kFlRows * 512 bytes.
+template <int D>
+__global__ void __launch_bounds__(kFlWarps * 32, 4)
 k_bprmf_flash(const float* __restrict__ U, const int64_t* __restrict__ uid, int64_t n_users,
               const float* __restrict__ T, const int64_t* __restrict__ ids, int64_t n_t,
               float* __restrict__ pred, float* __restrict__ gout, float* __restrict__ row_loss,
               float* __restrict__ dQ, float* __restrict__ qout, int B, int C, int cpad, int32_t* err_flag,
-              float* __restrict__ loss_out, unsigned int* __restrict__ done_counter,
-              const __grid_constant__ DirectPlanDev plan_i, const __grid_constant__ DirectPlanDev plan_u) {
-    constexpr int LPR = D / (4 * VPL);
+              float* __restrict__ loss_out, unsigned int* __restrict__ done_counter) {
+    constexpr int RCH = kFlRows, ST = kFlStages;
+    constexpr int LPR = D / 4;
     constexpr int GPW = 32 / LPR;                 // lane groups (rows in parallel) per warp
     constexpr int RS = LPR / RCH;                 // lanes holding a copy of one row's score after the multi-sum
     static_assert(LPR >= 1 && LPR <= 32 && RCH <= LPR && (RCH & (RCH - 1)) == 0, "shape");
-    constexpr int STAGE_F4 = RCH * VPL * 32;      // float4 per stage per warp
+    constexpr int STAGE_F4 = RCH * 32;            // float4 per stage per warp
     extern __shared__ __align__(16) unsigned char fl_smem[];
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
     const int sub = lane % LPR, grp = lane / LPR;
-    // per-warp regions: ring [ST][RCH][VPL][32] float4, then cpad floats of scores, then cpad row indices
+    // per-warp regions: ring [ST][RCH][32] float4, then cpad floats of scores, then cpad row indices
     unsigned char* wbase = fl_smem + (size_t)warp * ((size_t)ST * STAGE_F4 * 16 + (size_t)cpad * 8);
     float4* ring = reinterpret_cast<float4*>(wbase);
     float* xs = reinterpret_cast<float*>(wbase + (size_t)ST * STAGE_F4 * 16);
     uint32_t* sid = reinterpret_cast<uint32_t*>(xs + cpad);
     const float invB = 1.f / (float)B;
-    if (PLAN && blockIdx.x == 0 && threadIdx.x == 0) {
-        // counters the sort kernel of this step accumulates into (big-area cursor, long rows, row heads); the spill
-        // counter [0] was zeroed by the previous step's update kernel
-        plan_i.counters[1] = plan_i.counters[2] = plan_i.counters[3] = 0;
-        plan_u.counters[1] = plan_u.counters[2] = plan_u.counters[3] = 0;
-    }
 
-    for (int64_t b = (int64_t)blockIdx.x * WPC + warp; b < B; b += (int64_t)gridDim.x * WPC) {
+    for (int64_t b = (int64_t)blockIdx.x * kFlWarps + warp; b < B; b += (int64_t)gridDim.x * kFlWarps) {
         // ---- ids of the sample: one coalesced pass, range-checked once, parked as 32-bit row indices -------------
         const int64_t* idp = ids + b * C;
-        for (int c = lane; c < C; c += 32) {
-            const uint32_t key = (uint32_t)checked_id(idp[c], n_t, err_flag);
-            sid[c] = key;
-            if (PLAN) direct_scatter(plan_i, key, (uint32_t)(b * C + c));
-        }
+        for (int c = lane; c < C; c += 32) sid[c] = (uint32_t)checked_id(idp[c], n_t, err_flag);
         const int64_t qrow = checked_id(uid[b], n_users, lane == 0 ? err_flag : nullptr);
-        if (PLAN && lane == 0) direct_scatter(plan_u, (uint32_t)qrow, (uint32_t)b);
         __syncwarp();
-        float4 q[VPL];
-        float pp = 0.f;
         const float* r0p = T + (size_t)sid[0] * D + sub * 4;              // the positive's row (every group: same bytes)
-#pragma unroll
-        for (int v = 0; v < VPL; ++v) {
-            q[v] = ld4(U + qrow * D + (v * LPR + sub) * 4);
-            pp += dot4(q[v], ld4(r0p + v * LPR * 4));                     // not kept: re-read (L2) for dQ at the end
-        }
+        const float4 q = ld4(U + qrow * D + sub * 4);
+        const float pp = 0.f + dot4(q, ld4(r0p));                         // r0 not kept: re-read (L2) for dQ at the end
         // negatives of this group: c = 1 + grp + GPW * k, k = 0 .. ; chunk j covers k in [j * RCH, (j + 1) * RCH)
         const int nneg = C - 1;
         const int nch = (nneg + GPW * RCH - 1) / (GPW * RCH);               // chunks per group (warp-uniform)
@@ -138,9 +117,7 @@ k_bprmf_flash(const float* __restrict__ U, const int64_t* __restrict__ uid, int6
                 for (int r = 0; r < RCH; ++r) {
                     const int c = 1 + grp + GPW * (j * RCH + r);
                     const bool ok = c < C;
-                    const float* src = T + (size_t)sid[ok ? c : 0] * D + sub * 4;
-#pragma unroll
-                    for (int v = 0; v < VPL; ++v) fl_cp16(st + (r * VPL + v) * 32, src + v * LPR * 4, ok);
+                    fl_cp16(st + r * 32, T + (size_t)sid[ok ? c : 0] * D + sub * 4, ok);
                 }
             }
             asm volatile("cp.async.commit_group;\n" ::: "memory");        // one (possibly empty) group per call
@@ -148,17 +125,13 @@ k_bprmf_flash(const float* __restrict__ U, const int64_t* __restrict__ uid, int6
 #pragma unroll
         for (int j = 0; j < ST - 1; ++j) issue(j, j);
 
-        if (qout != nullptr && grp == 0) {
-#pragma unroll
-            for (int v = 0; v < VPL; ++v) st4(qout + b * D + (v * LPR + sub) * 4, q[v]);
-        }
+        if (qout != nullptr && grp == 0) st4(qout + b * D + sub * 4, q);
         const float p = group_sum<LPR>(pp);                               // positive's score, known to every group
         if (lane == 0) xs[0] = p;
 
         float M = -INFINITY, Zl = 0.f, Al = 0.f, Dl = 0.f;                 // running max; per-lane partial sums
-        float4 acc1[VPL], acc2[VPL];                                      // sum e s^2 r, sum e r (this lane's bytes)
-#pragma unroll
-        for (int v = 0; v < VPL; ++v) acc1[v] = acc2[v] = make_float4(0.f, 0.f, 0.f, 0.f);
+        float4 acc1 = make_float4(0.f, 0.f, 0.f, 0.f);                    // sum e s^2 r (this lane's bytes)
+        float4 acc2 = make_float4(0.f, 0.f, 0.f, 0.f);                    // sum e r
         int stage = 0, stage_in = ST - 1;
         for (int j = 0; j < nch; ++j) {
             issue(j + ST - 1, stage_in);
@@ -166,17 +139,12 @@ k_bprmf_flash(const float* __restrict__ U, const int64_t* __restrict__ uid, int6
             asm volatile("cp.async.wait_group %0;\n" ::"n"(ST - 1) : "memory");
             const float4* st = ring + stage * STAGE_F4 + lane;
             stage = (stage + 1 == ST) ? 0 : stage + 1;
-            float4 r[RCH][VPL];
+            float4 r[RCH];
             float d[RCH];
 #pragma unroll
             for (int k = 0; k < RCH; ++k) {
-                float a = 0.f;
-#pragma unroll
-                for (int v = 0; v < VPL; ++v) {
-                    r[k][v] = st[(k * VPL + v) * 32];
-                    a += dot4(q[v], r[k][v]);
-                }
-                d[k] = a;
+                r[k] = st[k * 32];
+                d[k] = 0.f + dot4(q, r[k]);
             }
             const float x = fl_group_sum_multi<LPR, RCH>(d, sub);          // score of row sub / RS of this chunk
             const int c_mine = 1 + grp + GPW * (j * RCH + sub / RS);
@@ -189,11 +157,8 @@ k_bprmf_flash(const float* __restrict__ U, const int64_t* __restrict__ uid, int6
                 const float sc = (Mn == -INFINITY) ? 1.f : __expf(M - Mn); // M = -inf -> 0: nothing accumulated yet
                 M = Mn;
                 Zl *= sc; Al *= sc; Dl *= sc;
-#pragma unroll
-                for (int v = 0; v < VPL; ++v) {
-                    acc1[v].x *= sc; acc1[v].y *= sc; acc1[v].z *= sc; acc1[v].w *= sc;
-                    acc2[v].x *= sc; acc2[v].y *= sc; acc2[v].z *= sc; acc2[v].w *= sc;
-                }
+                acc1.x *= sc; acc1.y *= sc; acc1.z *= sc; acc1.w *= sc;
+                acc2.x *= sc; acc2.y *= sc; acc2.z *= sc; acc2.w *= sc;
             }
             const float e = valid ? __expf(x - M) : 0.f;
             const float s = __fdividef(1.f, 1.f + __expf(x - p));
@@ -208,11 +173,8 @@ k_bprmf_flash(const float* __restrict__ U, const int64_t* __restrict__ uid, int6
             for (int k = 0; k < RCH; ++k) {
                 const float ek = __shfl_sync(B2R_FULL_MASK, e, k * RS, LPR);
                 const float wk = __shfl_sync(B2R_FULL_MASK, ess, k * RS, LPR);
-#pragma unroll
-                for (int v = 0; v < VPL; ++v) {
-                    fma4(acc2[v], ek, r[k][v]);
-                    fma4(acc1[v], wk, r[k][v]);
-                }
+                fma4(acc2, ek, r[k]);
+                fma4(acc1, wk, r[k]);
             }
         }
         asm volatile("cp.async.wait_group 0;\n" ::: "memory");
@@ -231,19 +193,16 @@ k_bprmf_flash(const float* __restrict__ U, const int64_t* __restrict__ uid, int6
                 A += __shfl_xor_sync(B2R_FULL_MASK, A, o);
                 Dp += __shfl_xor_sync(B2R_FULL_MASK, Dp, o);
             }
+            float* a1 = &acc1.x;
+            float* a2 = &acc2.x;
 #pragma unroll
-            for (int v = 0; v < VPL; ++v) {
-                float* a1 = &acc1[v].x;
-                float* a2 = &acc2[v].x;
+            for (int i = 0; i < 4; ++i) {
+                a1[i] *= sg;
+                a2[i] *= sg;
 #pragma unroll
-                for (int i = 0; i < 4; ++i) {
-                    a1[i] *= sg;
-                    a2[i] *= sg;
-#pragma unroll
-                    for (int o = LPR; o < 32; o <<= 1) {
-                        a1[i] += __shfl_xor_sync(B2R_FULL_MASK, a1[i], o);
-                        a2[i] += __shfl_xor_sync(B2R_FULL_MASK, a2[i], o);
-                    }
+                for (int o = LPR; o < 32; o <<= 1) {
+                    a1[i] += __shfl_xor_sync(B2R_FULL_MASK, a1[i], o);
+                    a2[i] += __shfl_xor_sync(B2R_FULL_MASK, a2[i], o);
                 }
             }
             M = Mall;
@@ -255,16 +214,13 @@ k_bprmf_flash(const float* __restrict__ U, const int64_t* __restrict__ uid, int6
         const float g0 = dS * Dp * invZ;
         const float kz = dS * invZ;
         if (grp == 0) {
-#pragma unroll
-            for (int v = 0; v < VPL; ++v) {
-                const float4 r0 = ld4(r0p + v * LPR * 4);
-                float4 o;
-                o.x = fmaf(g0, r0.x, kz * fmaf(-S, acc2[v].x, acc1[v].x));
-                o.y = fmaf(g0, r0.y, kz * fmaf(-S, acc2[v].y, acc1[v].y));
-                o.z = fmaf(g0, r0.z, kz * fmaf(-S, acc2[v].z, acc1[v].z));
-                o.w = fmaf(g0, r0.w, kz * fmaf(-S, acc2[v].w, acc1[v].w));
-                st4(dQ + b * D + (v * LPR + sub) * 4, o);
-            }
+            const float4 r0 = ld4(r0p);
+            float4 o;
+            o.x = fmaf(g0, r0.x, kz * fmaf(-S, acc2.x, acc1.x));
+            o.y = fmaf(g0, r0.y, kz * fmaf(-S, acc2.y, acc1.y));
+            o.z = fmaf(g0, r0.z, kz * fmaf(-S, acc2.z, acc1.z));
+            o.w = fmaf(g0, r0.w, kz * fmaf(-S, acc2.w, acc1.w));
+            st4(dQ + b * D + sub * 4, o);
         }
         if (lane == 0) row_loss[b] = -logf(fminf(fmaxf(S, 1e-8f), 1.f - 1e-8f));
         __syncwarp();                                                      // xs[] complete
@@ -287,8 +243,10 @@ k_bprmf_flash(const float* __restrict__ U, const int64_t* __restrict__ uid, int6
 
     // mean of the per-sample losses by the last CTA to finish (fixed summation order -> deterministic)
     if (loss_out != nullptr) {
+        constexpr int NT = kFlWarps * 32;
         __shared__ bool last;
-        __shared__ float red[256];
+        __shared__ float red[NT];
+        static_assert((NT & (NT - 1)) == 0, "tree reduction over a power of two");
         __threadfence();
         __syncthreads();
         if (threadIdx.x == 0) last = (atomicAdd(done_counter, 1u) == gridDim.x - 1);
@@ -296,17 +254,16 @@ k_bprmf_flash(const float* __restrict__ U, const int64_t* __restrict__ uid, int6
         if (last) {
             __threadfence();
             float a = 0.f;
-            for (int i = threadIdx.x; i < B; i += WPC * 32) a += __ldcg(row_loss + i);
+            for (int i = threadIdx.x; i < B; i += NT) a += __ldcg(row_loss + i);
             red[threadIdx.x] = a;
-            for (int i = WPC * 32 + threadIdx.x; i < 256; i += WPC * 32) red[i] = 0.f;
             __syncthreads();
-            for (int o = 128; o > 0; o >>= 1) {
+            for (int o = NT / 2; o > 0; o >>= 1) {
                 if ((int)threadIdx.x < o) red[threadIdx.x] += red[threadIdx.x + o];
                 __syncthreads();
             }
             if (threadIdx.x == 0) {
                 loss_out[0] = red[0] / (float)B;
-                *done_counter = 0u;
+                *done_counter = 0u;                                        // ready for the next launch
             }
         }
     }
@@ -316,63 +273,57 @@ k_bprmf_flash(const float* __restrict__ U, const int64_t* __restrict__ uid, int6
 
 using namespace b2r;
 
-// returns B2R_E_UNSUPPORTED when the shape is outside the kernel's class (d in {32, 64, 128}, C <= 1024).
-// plan_i / plan_u (both or neither): direct index plans of the item / user table that the kernel fills on the way.
-int b2r_bprmf_flash_launch(const float* U, const int64_t* uid, int64_t n_users, const float* I, const int64_t* iid,
-                           int64_t n_items, float* pred, float* grad_pred, float* row_loss, float* dQ, float* qout,
-                           int B, int C, int d, int32_t* err_flag, float* loss_out, unsigned int* done_counter,
-                           const DirectPlanDev* plan_i, const DirectPlanDev* plan_u, b2r_stream_t stream) {
+static int flash_launch(const float* U, const int64_t* uid, int64_t n_users, const float* I, const int64_t* iid,
+                        int64_t n_items, float* pred, float* grad_pred, float* row_loss, float* dQ, float* qout, int B,
+                        int C, int d, int32_t* err_flag, float* loss_out, unsigned int* done_counter, b2r_stream_t stream) {
+    B2R_REQUIRE(U && uid && I && iid && grad_pred && row_loss && dQ, B2R_E_BADARG, "b2r_bprmf_fused_fwd_bwd: null pointer");
+    B2R_REQUIRE(B > 0 && C > 0, B2R_E_BADARG, "b2r_bprmf_fused_fwd_bwd: B=%d C=%d", B, C);
+    B2R_REQUIRE(aligned16(U) && aligned16(I) && aligned16(dQ), B2R_E_BADARG, "b2r_bprmf_fused_fwd_bwd: alignment");
+    // row indices travel as 32-bit values (sid, checked against n_t) and flat positions b * C + c stay below 2^32 - 1
     if (!(d == 32 || d == 64 || d == 128) || C > 1024 || n_items >= 0xffffffffLL || n_users >= 0xffffffffLL ||
         (int64_t)B * C >= 0xffffffffLL)
-        return set_error(B2R_E_UNSUPPORTED, "bprmf_flash: d=%d C=%d", d, C);
+        return set_error(B2R_E_UNSUPPORTED, "b2r_bprmf_fused_fwd_bwd: d=%d C=%d", d, C);
     const int cpad = (C + 3) / 4 * 4;
-    // B2R_FLASH_WARPS=7 (A/B): 7 samples per CTA instead of 8 (leaves shared memory for co-resident plan CTAs; measured
-    // slower: 0.159 vs 0.151 ms per config-2 step)
-    static const int wpc = [] { const char* e = getenv("B2R_FLASH_WARPS"); return (e && atoi(e) == 7) ? 7 : 8; }();
-    const int64_t need = ((int64_t)B + wpc - 1) / wpc;
+    const int64_t need = ((int64_t)B + kFlWarps - 1) / kFlWarps;
     const int64_t cap = (int64_t)sm_count() * 32;                         // beyond that, warps loop over samples
     const int grid = (int)(need < cap ? need : cap);
-    const bool plan = plan_i != nullptr && plan_u != nullptr;
-    const DirectPlanDev none{};
-    const DirectPlanDev pi = plan ? *plan_i : none, pu = plan ? *plan_u : none;
-    // variant knob for A/B runs: B2R_FLASH="<VPL><RCH><ST>".  Default 143 (one float4 per lane, 4 rows per group per chunk,
-    // 3 stages: 0.1501 ms per config-2 step); 223 / 243 (two float4 per lane) execute fewer instructions but spill under
-    // the 64-register cap the single-wave residency needs and measure 0.152 ms (profiles/README r2).
-    static const int variant = [] { const char* e = getenv("B2R_FLASH"); return e ? atoi(e) : 143; }();
-#define B2R_FLW(D_, VPL, RCH, ST, PLAN, WPC)                                                                         \
+    const int smem = kFlWarps * (kFlStages * kFlRows * 32 * 16 + cpad * 8);
+#define B2R_FLASH_LAUNCH(D_)                                                                                         \
     do {                                                                                                             \
-        const int smem = WPC * (ST * RCH * VPL * 32 * 16 + cpad * 8);                                                \
         static int attr_smem = 0;                                                                                    \
         if (smem > attr_smem) {                                                                                      \
-            B2R_CUDA_OK(cudaFuncSetAttribute(k_bprmf_flash<D_, VPL, RCH, ST, PLAN, WPC>,                             \
-                                             cudaFuncAttributeMaxDynamicSharedMemorySize, smem));                    \
+            B2R_CUDA_OK(cudaFuncSetAttribute(k_bprmf_flash<D_>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem)); \
             attr_smem = smem;                                                                                        \
         }                                                                                                            \
-        k_bprmf_flash<D_, VPL, RCH, ST, PLAN, WPC><<<grid, WPC * 32, smem, as_stream(stream)>>>(                     \
+        k_bprmf_flash<D_><<<grid, kFlWarps * 32, smem, as_stream(stream)>>>(                                         \
             U, uid, n_users, I, iid, n_items, pred, grad_pred, row_loss, dQ, qout, B, C, cpad, err_flag, loss_out,   \
-            done_counter, pi, pu);                                                                                   \
+            done_counter);                                                                                           \
     } while (0)
-#define B2R_FL(D_, VPL, RCH, ST, PLAN)                                                                               \
-    do {                                                                                                             \
-        if (wpc == 8) B2R_FLW(D_, VPL, RCH, ST, PLAN, 8); else B2R_FLW(D_, VPL, RCH, ST, PLAN, 7);                   \
-    } while (0)
-#define B2R_FL_V(D_, PLAN)                                                                                           \
-    do {                                                                                                             \
-        if (variant == 223) B2R_FL(D_, 2, 2, 3, PLAN);                                                               \
-        else if (variant == 243) B2R_FL(D_, 2, 4, 3, PLAN);                                                          \
-        else B2R_FL(D_, 1, 4, 3, PLAN);                                                                              \
-    } while (0)
-#define B2R_FL_D(D_)                                                                                                 \
-    do {                                                                                                             \
-        if (plan) B2R_FL_V(D_, true); else B2R_FL_V(D_, false);                                                      \
-    } while (0)
-    if (d == 32) B2R_FL_D(32);
-    else if (d == 64) B2R_FL_D(64);
-    else B2R_FL_D(128);
-#undef B2R_FL_D
-#undef B2R_FL_V
-#undef B2R_FL
-#undef B2R_FLW
+    switch (d) {
+        case 32: B2R_FLASH_LAUNCH(32); break;
+        case 64: B2R_FLASH_LAUNCH(64); break;
+        default: B2R_FLASH_LAUNCH(128); break;
+    }
+#undef B2R_FLASH_LAUNCH
     B2R_LAUNCH_OK("k_bprmf_flash");
     return 0;
+}
+
+extern "C" int b2r_bprmf_fused_fwd_bwd(const float* U, const int64_t* uid, int64_t n_users, const float* I,
+                                       const int64_t* iid, int64_t n_items, float* pred, float* grad_pred,
+                                       float* row_loss, float* dQ, int B, int C, int d, int32_t* err_flag,
+                                       b2r_stream_t stream) {
+    return flash_launch(U, uid, n_users, I, iid, n_items, pred, grad_pred, row_loss, dQ, nullptr, B, C, d, err_flag, nullptr,
+                        nullptr, stream);
+}
+
+// same, and the mean loss is produced by the kernel itself (done_counter: a zero-initialised device word the kernel
+// leaves zero again) and the gathered user rows are kept (qout [B, d]: the item-side gradient's source, so that the
+// user table may be updated while the item table still is); used by the step context
+int b2r_bprmf_fused_fwd_bwd_loss(const float* U, const int64_t* uid, int64_t n_users, const float* I, const int64_t* iid,
+                                 int64_t n_items, float* grad_pred, float* row_loss, float* dQ, float* qout, int B, int C,
+                                 int d, int32_t* err_flag, float* loss_out, unsigned int* done_counter,
+                                 b2r_stream_t stream) {
+    return flash_launch(U, uid, n_users, I, iid, n_items, nullptr, grad_pred, row_loss, dQ, qout, B, C, d, err_flag, loss_out,
+                        done_counter, stream);
 }

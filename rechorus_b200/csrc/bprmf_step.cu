@@ -1,43 +1,26 @@
 // bprmf_step.cu -- one whole BPRMF training step enqueued from C (b2r_bprmf_train_step) on a step context.
 //
 // Stream plan (step t):
-//   main :  fused gather+score+loss+dQ (rows read once) -> mean(loss) -> [wait plan(t)] -> segment+opt(I) -> segment+opt(U)
+//   main :  fused gather+score+loss+dQ (rows read once) -> mean(loss) -> [wait plan(t)] -> opt(I) + opt(U) in one launch
 //   side :  plan(t+1) for the NEXT batch's ids (or plan(t) itself when nothing was prefetched)
-// The index plan (radix sort of the ids) only depends on the ids, so the context builds it one step ahead on
+// The index plan (per-bucket sort of the ids) only depends on the ids, so the context builds it one step ahead on
 // a library-owned non-blocking stream while the HBM-bound kernels of the current step run; joins are event
-// waits, never host synchronisations.  Plans (bucket partitions, bucket.cu) are double-buffered in the caller-provided
-// workspace.  d must be 32, 64 or 128 (the widths the bucket kernels are built for).
-#include <stdlib.h>
-
+// waits, never host synchronisations.  Plans (direct plans, plan_direct.cuh) are double-buffered in the caller-provided
+// workspace.  d must be 32, 64 or 128 (the widths the plan's apply kernel is built for).  Shapes the streaming forward
+// kernel does not take (C > 1024) run the unfused gather / rowdot / loss / query-backward kernels instead.
 #include "common.cuh"
 #include "plan_direct.cuh"
-
-extern "C" int b2r_bprmf_fused_fwd_bwd(const float* U, const int64_t* uid, int64_t n_users, const float* I,
-                                       const int64_t* iid, int64_t n_items, float* pred, float* grad_pred,
-                                       float* row_loss, float* dQ, int B, int C, int d, int32_t* err_flag,
-                                       b2r_stream_t stream);
 
 int b2r_bprmf_fused_fwd_bwd_loss(const float* U, const int64_t* uid, int64_t n_users, const float* I, const int64_t* iid,
                                  int64_t n_items, float* grad_pred, float* row_loss, float* dQ, float* qout, int B, int C,
                                  int d, int32_t* err_flag, float* loss_out, unsigned int* done_counter,
                                  b2r_stream_t stream);
 
-int b2r_bprmf_flash_launch(const float* U, const int64_t* uid, int64_t n_users, const float* I, const int64_t* iid,
-                           int64_t n_items, float* pred, float* grad_pred, float* row_loss, float* dQ, float* qout,
-                           int B, int C, int d, int32_t* err_flag, float* loss_out, unsigned int* done_counter,
-                           const b2r::DirectPlanDev* plan_i, const b2r::DirectPlanDev* plan_u, b2r_stream_t stream);
-
 namespace b2r {
-
-struct PlanBuf {
-    size_t iws, uws;                 // bucket workspaces (b2r_bucket_partition) for the item / user table
-};
 
 struct StepLayout {
     size_t q, pred, g, rows, dQ, counter;
-    PlanBuf plan[2];
-    size_t iws_bytes, uws_bytes;
-    size_t dir_i[2], dir_u[2], dir_i_bytes, dir_u_bytes; // direct plans (plan_direct.cuh), double-buffered; 0: not available
+    size_t dir_i[2], dir_u[2], dir_i_bytes, dir_u_bytes; // direct plans (plan_direct.cuh), double-buffered
     size_t total;
 };
 
@@ -55,21 +38,14 @@ static bool step_layout(int B, int C, int d, int64_t n_users, int64_t n_items, S
     L->rows = take((size_t)B * 4);
     L->dQ = take((size_t)B * d * 4);
     L->counter = take(256);
-    L->iws_bytes = b2r_bucket_workspace_bytes((int64_t)n, n_items);
-    L->uws_bytes = b2r_bucket_workspace_bytes(B, n_users);
-    for (int s = 0; s < 2; ++s) {
-        L->plan[s].iws = take(L->iws_bytes);
-        L->plan[s].uws = take(L->uws_bytes);
-    }
     L->dir_i_bytes = direct_workspace_bytes((int64_t)n, n_items);
     L->dir_u_bytes = direct_workspace_bytes(B, n_users);
-    if (L->dir_i_bytes == 0 || L->dir_u_bytes == 0) L->dir_i_bytes = L->dir_u_bytes = 0;
     for (int sl = 0; sl < 2; ++sl) {
         L->dir_i[sl] = take(L->dir_i_bytes);
         L->dir_u[sl] = take(L->dir_u_bytes);
     }
     L->total = off;
-    return L->iws_bytes != 0 && L->uws_bytes != 0;
+    return L->dir_i_bytes != 0 && L->dir_u_bytes != 0;
 }
 
 struct StepCtx {
@@ -83,9 +59,6 @@ struct StepCtx {
     const void* pre_uid;
     const void* pre_iid;
     bool have_pre;
-    int mode;                         // 0: direct plans built one batch ahead on the side stream (default);
-                                      // 1: the forward kernel fills the direct plans itself, one stream (B2R_STEP=inline);
-                                      // 2: count / scan / scatter / sort bucket plans one batch ahead (B2R_STEP=legacy)
 };
 
 }  // namespace b2r
@@ -124,10 +97,7 @@ extern "C" int b2r_bprmf_ctx_create(void** ctx_out, int B, int C, int d, int64_t
     // the next batch is starved and the next step's update waits for it (measured: 0.177 vs 0.199 ms per step).
     int prio_lo = 0, prio_hi = 0;
     cudaError_t e = cudaDeviceGetStreamPriorityRange(&prio_lo, &prio_hi);
-    // B2R_SIDE_PRIO=low (A/B knob): plan stream at the lowest priority instead
-    const char* sp = getenv("B2R_SIDE_PRIO");
-    const int side_prio = (sp && sp[0] == 'l') ? prio_lo : prio_hi;
-    if (e == cudaSuccess) e = cudaStreamCreateWithPriority(&c->side, cudaStreamNonBlocking, side_prio);
+    if (e == cudaSuccess) e = cudaStreamCreateWithPriority(&c->side, cudaStreamNonBlocking, prio_hi);
     if (e == cudaSuccess) e = cudaEventCreateWithFlags(&c->fork, cudaEventDisableTiming);
     if (e == cudaSuccess) e = cudaEventCreateWithFlags(&c->join[0], cudaEventDisableTiming);
     if (e == cudaSuccess) e = cudaEventCreateWithFlags(&c->join[1], cudaEventDisableTiming);
@@ -140,29 +110,14 @@ extern "C" int b2r_bprmf_ctx_create(void** ctx_out, int B, int C, int d, int64_t
         delete c;
         return set_error((int)e, "b2r_bprmf_ctx_create: %s", cudaGetErrorString(e));
     }
-    for (int sl = 0; sl < 2; ++sl) {      // bucket counters start at zero (the scan kernel re-zeroes them every step)
-        int rc = b2r_bucket_workspace_init(c->ws + c->L.plan[sl].iws, c->L.iws_bytes, (int64_t)B * C, n_items, c->side);
-        if (rc == 0) rc = b2r_bucket_workspace_init(c->ws + c->L.plan[sl].uws, c->L.uws_bytes, B, n_users, c->side);
+    // Index plans: "direct" plans (plan_direct.cuh: one scatter launch into fixed-capacity bucket regions, one sort launch,
+    // both tables per launch) built for the NEXT batch on the high-priority side stream underneath this step's kernels.
+    for (int sl = 0; sl < 2; ++sl) {
+        int rc = direct_workspace_init(c->ws + c->L.dir_i[sl], c->L.dir_i_bytes, (int64_t)B * C, n_items, c->side);
+        if (rc == 0) rc = direct_workspace_init(c->ws + c->L.dir_u[sl], c->L.dir_u_bytes, B, n_users, c->side);
         if (rc != 0) {
             delete c;
             return rc;
-        }
-    }
-    // Index plans.  Default (mode 0): "direct" plans (plan_direct.cuh: one scatter launch into fixed-capacity bucket regions,
-    // one sort launch, both tables per launch) built for the NEXT batch on the high-priority side stream underneath this
-    // step's kernels.  B2R_STEP=inline (mode 1): the forward kernel scatters the pairs itself, everything on one stream.
-    // B2R_STEP=legacy (mode 2): the round-1 form, count / scan / scatter / sort per table (8 launches) one batch ahead.
-    const char* mode = getenv("B2R_STEP");
-    c->mode = (mode && mode[0] == 'i') ? 1 : ((mode && mode[0] == 'l') ? 2 : 0);
-    if (c->L.dir_i_bytes == 0) c->mode = 2;
-    if (c->mode != 2) {
-        for (int sl = 0; sl < 2; ++sl) {
-            int rc = direct_workspace_init(c->ws + c->L.dir_i[sl], c->L.dir_i_bytes, (int64_t)B * C, n_items, c->side);
-            if (rc == 0) rc = direct_workspace_init(c->ws + c->L.dir_u[sl], c->L.dir_u_bytes, B, n_users, c->side);
-            if (rc != 0) {
-                delete c;
-                return rc;
-            }
         }
     }
     e = cudaStreamSynchronize(c->side);
@@ -196,25 +151,13 @@ extern "C" int b2r_bprmf_ctx_reset(void* ctx) {
 
 static int build_plans(StepCtx* c, int slot, const int64_t* uid, const int64_t* iid, int32_t* err_flag) {
     char* base = c->ws;
-    if (c->mode == 0) {
-        const int64_t nn = (int64_t)c->B * c->C;
-        profile_begin(B2R_PROF_PLAN_I, c->side);
-        int rc = direct_scatter_pair(iid, nn, c->n_items, base + c->L.dir_i[slot], uid, c->B, c->n_users,
-                                     base + c->L.dir_u[slot], err_flag, c->side);
-        if (rc == 0) rc = direct_sort_pair(base + c->L.dir_i[slot], nn, c->n_items, base + c->L.dir_u[slot], c->B, c->n_users, c->side);
-        if (rc != 0) return rc;
-        profile_end(B2R_PROF_PLAN_I, c->side);
-        B2R_CUDA_OK(cudaEventRecord(c->join[slot], c->side));
-        return 0;
-    }
-    const PlanBuf& p = c->L.plan[slot];
     const int64_t n = (int64_t)c->B * c->C;
     profile_begin(B2R_PROF_PLAN_I, c->side);
-    int rc = b2r_bucket_partition(iid, n, c->n_items, -1, 0, base + p.iws, c->L.iws_bytes, err_flag, c->side);
+    int rc = direct_scatter_pair(iid, n, c->n_items, base + c->L.dir_i[slot], uid, c->B, c->n_users,
+                                 base + c->L.dir_u[slot], err_flag, c->side);
+    if (rc == 0) rc = direct_sort_pair(base + c->L.dir_i[slot], n, c->n_items, base + c->L.dir_u[slot], c->B, c->n_users, c->side);
     if (rc != 0) return rc;
     profile_end(B2R_PROF_PLAN_I, c->side);
-    rc = b2r_bucket_partition(uid, c->B, c->n_users, -1, 0, base + p.uws, c->L.uws_bytes, err_flag, c->side);
-    if (rc != 0) return rc;
     B2R_CUDA_OK(cudaEventRecord(c->join[slot], c->side));
     return 0;
 }
@@ -236,34 +179,6 @@ extern "C" int b2r_bprmf_train_step(void* ctx, const b2r_bprmf_tables* t, const 
     const int64_t n = (int64_t)B * C;
     int rc;
 
-    if (c->mode == 1) {
-        // forward (+ plan pairs) -> per-bucket sort of both plans -> update of both tables: three launches, one stream
-        float* q = reinterpret_cast<float*>(base + c->L.q);
-        const DirectPlanDev pi = direct_plan_dev(base + c->L.dir_i[0], n, c->n_items);
-        const DirectPlanDev pu = direct_plan_dev(base + c->L.dir_u[0], B, c->n_users);
-        profile_begin(B2R_PROF_SCORE_FWD, main_s);
-        rc = b2r_bprmf_flash_launch(t->U, uid, t->n_users, t->I, iid, t->n_items, nullptr, g, rows, dQ, q, B, C, d, err_flag,
-                                    loss_out, reinterpret_cast<unsigned int*>(base + c->L.counter), &pi, &pu, main_s);
-        if (rc == 0) {
-            profile_end(B2R_PROF_SCORE_FWD, main_s);
-            profile_begin(B2R_PROF_PLAN_I, main_s);
-            rc = direct_sort_pair(base + c->L.dir_i[0], n, c->n_items, base + c->L.dir_u[0], B, c->n_users, main_s);
-            if (rc != 0) return rc;
-            profile_end(B2R_PROF_PLAN_I, main_s);
-            const b2r_grad_source su{dQ, nullptr, nullptr, B, 1, 0};
-            const b2r_grad_source si{q, g, nullptr, n, C, 0};
-            const b2r_apply_job ji{base + c->L.dir_i[0], n, t->n_items, &si, nullptr, nullptr, t->I, t->Im, t->Iv};
-            const b2r_apply_job ju{base + c->L.dir_u[0], B, t->n_users, &su, nullptr, nullptr, t->U, t->Um, t->Uv};
-            profile_begin(B2R_PROF_SEGMENT_I, main_s);
-            rc = direct_apply_pair(&ji, &ju, d, 2, opt, main_s);
-            if (rc != 0) return rc;
-            profile_end(B2R_PROF_SEGMENT_I, main_s);
-            return 0;
-        }
-        if (rc != B2R_E_UNSUPPORTED) return rc;
-        c->mode = 2;                                        // shape outside the streaming kernel's class: legacy form
-    }
-
     // everything the side stream does from here on is ordered after what main has enqueued so far
     // (in particular after the previous step's readers of the plan buffer about to be overwritten)
     B2R_CUDA_OK(cudaEventRecord(c->fork, main_s));
@@ -274,11 +189,8 @@ extern "C" int b2r_bprmf_train_step(void* ctx, const b2r_bprmf_tables* t, const 
         rc = build_plans(c, cur, uid, iid, err_flag);     // nothing prefetched for this batch: build it now
         if (rc != 0) return rc;
     }
-    // B2R_PLAN_AFTER=1 (A/B knob): start the next batch's plan only when this step's forward kernel has finished, so that
-    // the plan's kernels share the SMs with the HBM-bound update kernel instead of with the single-wave forward kernel
-    static const bool plan_after = [] { const char* e = getenv("B2R_PLAN_AFTER"); return e && atoi(e) != 0; }();
     const bool prefetch = next_uid != nullptr && next_iid != nullptr;
-    if (prefetch && !plan_after) {
+    if (prefetch) {
         rc = build_plans(c, cur ^ 1, next_uid, next_iid, err_flag);
         if (rc != 0) return rc;
     }
@@ -311,23 +223,15 @@ extern "C" int b2r_bprmf_train_step(void* ctx, const b2r_bprmf_tables* t, const 
         profile_end(B2R_PROF_SCORE_BWDQ, main_s);
     }
 
-    if (prefetch && plan_after) {
-        B2R_CUDA_OK(cudaEventRecord(c->fork, main_s));                 // after the forward kernel(s)
-        B2R_CUDA_OK(cudaStreamWaitEvent(c->side, c->fork, 0));
-        rc = build_plans(c, cur ^ 1, next_uid, next_iid, err_flag);
-        if (rc != 0) return rc;
-    }
     // join plan(t); then the fused backward+optimizer on both tables in one launch: dI = g * q reads the saved user
     // rows, so the two updates are independent and the small user-table job runs underneath the item-table job
     B2R_CUDA_OK(cudaStreamWaitEvent(main_s, c->join[cur], 0));
-    const PlanBuf& p = c->L.plan[cur];
-    const bool dplan = c->mode == 0;
     const b2r_grad_source su{dQ, nullptr, nullptr, B, 1, 0};
     const b2r_grad_source si{q, g, nullptr, n, C, 0};
-    const b2r_apply_job ji{base + (dplan ? c->L.dir_i[cur] : p.iws), n, t->n_items, &si, nullptr, nullptr, t->I, t->Im, t->Iv};
-    const b2r_apply_job ju{base + (dplan ? c->L.dir_u[cur] : p.uws), B, t->n_users, &su, nullptr, nullptr, t->U, t->Um, t->Uv};
+    const b2r_apply_job ji{base + c->L.dir_i[cur], n, t->n_items, &si, nullptr, nullptr, t->I, t->Im, t->Iv};
+    const b2r_apply_job ju{base + c->L.dir_u[cur], B, t->n_users, &su, nullptr, nullptr, t->U, t->Um, t->Uv};
     profile_begin(B2R_PROF_SEGMENT_I, main_s);
-    rc = dplan ? direct_apply_pair(&ji, &ju, d, 2, opt, main_s) : b2r_bucket_apply_pair(&ji, &ju, d, 2, opt, main_s);
+    rc = direct_apply_pair(&ji, &ju, d, 2, opt, main_s);
     if (rc != 0) return rc;
     profile_end(B2R_PROF_SEGMENT_I, main_s);
     return 0;

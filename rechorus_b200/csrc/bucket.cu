@@ -1,13 +1,12 @@
 // bucket.cu -- the hot-path form of the row-sparse embedding backward + optimizer (K2b).
-//   plan side (depends only on the ids; runs on the step context's side stream, one step ahead):
-//     k_bucket_count / k_bucket_scan / k_bucket_scatter  partition the batch's (row id, position) pairs into buckets
-//         of 2^shift consecutive table rows (~200 pairs each): two passes over the ids with L2 atomics on
-//         line-padded counters;
-//     k_bucket_sort  one CTA per bucket sorts its pairs by (row, position) in shared memory (bitonic network) and
-//         writes them back in place.  Buckets cover ascending disjoint row ranges, so the whole array ends up
-//         sorted exactly as a device-wide radix sort would leave it, at a fraction of the cost; rows with many
-//         contributions are listed for the cooperative kernel; buckets beyond the shared-memory capacity are
-//         chunk-sorted and merged.
+//   plan side (depends only on the ids; runs on the step context's side stream, one step ahead; plan_direct.cuh):
+//     k_direct_scatter_pair  drops the batch's (row id, position) pairs into fixed-capacity regions of buckets of
+//         2^shift consecutive table rows (~200 pairs each) with one L2 atomic per pair on a line-padded cursor;
+//     k_bucket_sort_direct  one CTA per bucket sorts its pairs by (row, position) in shared memory (counting sort;
+//         bitonic network for rows with many contributions and wide buckets) and writes them back in place.  Buckets
+//         cover ascending disjoint row ranges, so the whole array ends up sorted exactly as a device-wide radix sort
+//         would leave it, at a fraction of the cost; rows with many contributions are listed for the cooperative
+//         reduction; buckets beyond the shared-memory capacity are chunk-sorted and merged.
 //         The sort also lists every touched row once: (row, first position, index of its first pair, run length).
 //   apply side (main stream):
 //     k_apply_sorted  one lane group per touched row (head list): requests w (m, v), sums the row's contributions in
@@ -17,8 +16,6 @@
 // Every sum has a fixed order whatever order the partition's atomics produced -> same bits on every run.
 // Replaces ATen embedding_dense_backward + the dense grad zero-fill + the embedding part of optimizer.step()
 // (helpers/BaseRunner.py:193,205,206).
-#include <stdlib.h>
-
 #include "common.cuh"
 #include "plan_direct.cuh"
 
@@ -36,7 +33,6 @@ struct BSrc {
 constexpr int kCap = 2048;        // pairs a CTA sorts in shared memory (16 KB)
 constexpr int kLong = 48;         // rows with at least this many contributions are reduced by the whole CTA
 constexpr int kBT = 256;
-constexpr int kPad = 32;          // ints per bucket counter: one 128-byte line each (L2 atomics serialise per line)
 constexpr int kCountShift = 12;   // counting-sort candidate: buckets of at most 4096 rows ...
 constexpr int kCountRows = 1 << kCountShift;
 constexpr int kRunMax = 32;       // ... whose longest row has at most this many contributions
@@ -74,84 +70,6 @@ __device__ __forceinline__ void b_optim(const b2r_optim& o, float4& w, float4& m
             vp[i] = fmaf(g, g, vp[i]);
             wp[i] = wp[i] - o.lr * g / (sqrtf(vp[i]) + o.eps);
         }
-    }
-}
-
-// ---------------------------------------------------------------------------------------------------
-// partition
-// ---------------------------------------------------------------------------------------------------
-__global__ void __launch_bounds__(kBT)
-k_bucket_count(const int64_t* __restrict__ ids, int64_t n, int64_t n_rows, int shift, int64_t ignore_id,
-               int64_t ignore_n, int* __restrict__ count, int32_t* err_flag) {
-    for (int64_t i = (int64_t)blockIdx.x * kBT + threadIdx.x; i < n; i += (int64_t)gridDim.x * kBT) {
-        const int64_t id = ids[i];
-        if (i < ignore_n && id == ignore_id) continue;
-        const int64_t key = checked_id(id, n_rows, err_flag);
-        atomicAdd(&count[(key >> shift) * kPad], 1);
-    }
-}
-
-// single CTA: off = exclusive scan(count); cursor = off; count = 0 (ready for the next step)
-__global__ void __launch_bounds__(1024)
-k_bucket_scan(int* __restrict__ count, int* __restrict__ cursor, int* __restrict__ off, int nb) {
-    __shared__ int wsum[32];
-    __shared__ int carry;
-    __shared__ int nbig;
-    if (threadIdx.x == 0) {
-        carry = 0;
-        nbig = 0;
-    }
-    __syncthreads();
-    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-    for (int base = 0; base < nb; base += 1024) {
-        const int i = base + threadIdx.x;
-        const int v = i < nb ? count[(int64_t)i * kPad] : 0;
-        if (v > kCap) atomicAdd(&nbig, 1);
-        int x = v;
-#pragma unroll
-        for (int o = 1; o < 32; o <<= 1) {
-            const int y = __shfl_up_sync(B2R_FULL_MASK, x, o);
-            if (lane >= o) x += y;
-        }
-        if (lane == 31) wsum[warp] = x;
-        __syncthreads();
-        if (warp == 0) {
-            int s = wsum[lane];
-#pragma unroll
-            for (int o = 1; o < 32; o <<= 1) {
-                const int y = __shfl_up_sync(B2R_FULL_MASK, s, o);
-                if (lane >= o) s += y;
-            }
-            wsum[lane] = s;
-        }
-        __syncthreads();
-        const int excl = carry + (warp > 0 ? wsum[warp - 1] : 0) + x - v;
-        if (i < nb) {
-            off[i] = excl;
-            cursor[(int64_t)i * kPad] = excl;
-            count[(int64_t)i * kPad] = 0;
-        }
-        __syncthreads();
-        if (threadIdx.x == 1023) carry += wsum[31];
-        __syncthreads();
-    }
-    if (threadIdx.x == 0) {
-        off[nb] = carry;
-        off[nb + 1] = nbig;          // number of buckets too large for the shared-memory sort (informational)
-        off[nb + 2] = 0;             // long-row counter, filled by k_bucket_sort
-        off[nb + 3] = 0;             // row-head counter, filled by k_bucket_sort
-    }
-}
-
-__global__ void __launch_bounds__(kBT)
-k_bucket_scatter(const int64_t* __restrict__ ids, int64_t n, int64_t n_rows, int shift, int64_t ignore_id,
-                 int64_t ignore_n, int* __restrict__ cursor, uint64_t* __restrict__ pairs) {
-    for (int64_t i = (int64_t)blockIdx.x * kBT + threadIdx.x; i < n; i += (int64_t)gridDim.x * kBT) {
-        const int64_t id = ids[i];
-        if (i < ignore_n && id == ignore_id) continue;
-        const int64_t key = (id < 0 || id >= n_rows) ? 0 : id;
-        const int slot = atomicAdd(&cursor[(key >> shift) * kPad], 1);
-        pairs[slot] = ((uint64_t)key << 32) | (uint64_t)(uint32_t)i;
     }
 }
 
@@ -245,13 +163,12 @@ __device__ __forceinline__ void emit_row_heads(const uint64_t* a, int cnt, int b
 }
 
 // ---------------------------------------------------------------------------------------------------
-// Counting sort of a bucket (the default; B2R_BUCKET_SORT=bitonic selects the network below instead).
-// The bitonic network costs 36-45 barrier-separated stages per bucket; a bucket's keys span only R = 2^shift rows, so
-// one shared-memory histogram over the rows gives every pair its row's start, an arrival-order slot inside the row,
-// and -- for free -- the row heads.  Rows with several contributions (a minority) are put in ascending position by
-// one thread each (insertion sort, at most kRunMax elements).  Returns false, having written nothing, when a row has
-// more than kRunMax contributions: the caller then runs the bitonic path.  Output is identical to the bitonic path
-// (same sorted array; the head list is a permutation of the same entries).
+// Counting sort of a bucket.  The bitonic network costs 36-45 barrier-separated stages per bucket; a bucket's keys span
+// only R = 2^shift rows, so one shared-memory histogram over the rows gives every pair its row's start, an arrival-order
+// slot inside the row, and -- for free -- the row heads.  Rows with several contributions (a minority) are put in
+// ascending position by one thread each (insertion sort, at most kRunMax elements).  Returns false, having written
+// nothing, when a row has more than kRunMax contributions: the caller then runs the bitonic path.  Output is identical
+// to the bitonic path (same sorted array; the head list is a permutation of the same entries).
 // ---------------------------------------------------------------------------------------------------
 __device__ __forceinline__ bool bucket_sort_counting(uint64_t* __restrict__ g, int cnt, int beg, uint32_t row0, int R,
                                                      uint64_t* s, int* hist, int* scratch, int* n_heads,
@@ -354,12 +271,11 @@ __device__ __forceinline__ bool bucket_sort_counting(uint64_t* __restrict__ g, i
 
 // sort one bucket's pairs g[0, cnt) in place (beg = index of g[0] in the plan's pair address space, tg = scratch of the
 // same extent for the merge path) and list its row heads / long rows
-template <bool COUNT>
 __device__ __forceinline__ void sort_one_bucket(uint64_t* g, uint64_t* tg, int cnt, int beg, uint32_t row0, int shift,
                                                 uint64_t* s, int* hist, int* scratch, int* head_cnt, int* head_base,
                                                 int* n_long, uint2* longs, int long_cap, int* n_heads, uint4* heads) {
     const int tid = threadIdx.x;
-    if (COUNT && cnt <= kCap && shift <= kCountShift &&
+    if (cnt <= kCap && shift <= kCountShift &&
         bucket_sort_counting(g, cnt, beg, row0, 1 << shift, s, hist, scratch, n_heads, heads))
         return;
     if (cnt <= kCap) {
@@ -408,37 +324,11 @@ __device__ __forceinline__ void sort_one_bucket(uint64_t* g, uint64_t* tg, int c
 }
 
 // ---------------------------------------------------------------------------------------------------
-// k_bucket_sort: one CTA per bucket sorts its (row, position) pairs in place.  Buckets cover ascending, disjoint
-// row ranges, so afterwards the whole pairs array is sorted by (row, position) -- the same order a device-wide
-// radix sort would give, at a fraction of its cost.  Rows with >= kLong contributions are listed for the
-// cooperative kernel.  Buckets larger than the shared-memory capacity (hot rows, tiny tables) are sorted in
-// kCap-sized chunks and then merged pairwise through the `tmp` array.
-// ---------------------------------------------------------------------------------------------------
-template <bool COUNT>
-__global__ void __launch_bounds__(kBT)
-k_bucket_sort(uint64_t* __restrict__ pairs, uint64_t* __restrict__ tmp, const int* __restrict__ off, int nb,
-              int* __restrict__ n_long, uint2* __restrict__ longs, int long_cap, int* __restrict__ n_heads,
-              uint4* __restrict__ heads, int shift) {
-    __shared__ uint64_t s[kCap];
-    __shared__ int head_cnt, head_base;
-    __shared__ int hist[COUNT ? kCountRows + 1 : 1];
-    __shared__ int scratch[COUNT ? 40 : 1];
-    if (threadIdx.x == 0) head_cnt = 0;
-    __syncthreads();
-    for (int b = blockIdx.x; b < nb; b += gridDim.x) {
-        const int beg = off[b];
-        const int cnt = off[b + 1] - beg;
-        if (cnt == 0) continue;
-        sort_one_bucket<COUNT>(pairs + beg, tmp + beg, cnt, beg, (uint32_t)b << shift, shift, s, hist, scratch, &head_cnt,
-                               &head_base, n_long, longs, long_cap, n_heads, heads);
-    }
-}
-
-// ---------------------------------------------------------------------------------------------------
-// k_bucket_sort_direct: the same per-bucket sort over plans whose pairs were dropped into fixed-capacity bucket regions
-// by the forward kernel (plan_direct.cuh).  A bucket that overflowed its region (skewed ids) first collects its spilled
-// pairs from the spill list into the "big" area behind the regions and is sorted there.  Cursors are left zero for the
-// next step.  Two plans (two tables of one step) ride in one launch.
+// k_bucket_sort_direct: one CTA per bucket sorts its (row, position) pairs in place (sort_one_bucket) over plans whose
+// pairs were dropped into fixed-capacity bucket regions by k_direct_scatter_pair (plan_direct.cuh).  A bucket that
+// overflowed its region (skewed ids) first collects its spilled pairs from the spill list into the "big" area behind
+// the regions and is sorted there.  Cursors are left zero for the next step.  Two plans (two tables of one step) ride in
+// one launch.
 // ---------------------------------------------------------------------------------------------------
 struct DirectSortJob {
     int nb, cap, shift, grid;
@@ -455,7 +345,6 @@ struct DirectSortJob {
     uint4* heads;
 };
 
-template <bool COUNT>
 __device__ __forceinline__ void direct_sort_job(const DirectSortJob& J, int bid, uint64_t* s, int* hist, int* scratch,
                                                 int* head_cnt, int* head_base, int* sh) {
     const int tid = threadIdx.x;
@@ -471,7 +360,7 @@ __device__ __forceinline__ void direct_sort_job(const DirectSortJob& J, int bid,
         const uint32_t row0 = (uint32_t)b << J.shift;
         if (raw <= J.cap) {
             const int beg = b * J.cap;
-            sort_one_bucket<COUNT>(J.region + (int64_t)beg, J.tmp, raw, beg, row0, J.shift, s, hist, scratch, head_cnt,
+            sort_one_bucket(J.region + (int64_t)beg, J.tmp, raw, beg, row0, J.shift, s, hist, scratch, head_cnt,
                                    head_base, J.counters + 2, J.longs, J.long_cap, J.counters + 3, J.heads);
             continue;
         }
@@ -499,7 +388,7 @@ __device__ __forceinline__ void direct_sort_job(const DirectSortJob& J, int bid,
         }
         __syncthreads();
         // pair indices of the big area continue after the regions: nb * cap + offset
-        sort_one_bucket<COUNT>(g, J.tmp + base, total, J.nb * J.cap + base, row0, J.shift, s, hist, scratch, head_cnt,
+        sort_one_bucket(g, J.tmp + base, total, J.nb * J.cap + base, row0, J.shift, s, hist, scratch, head_cnt,
                                head_base, J.counters + 2, J.longs, J.long_cap, J.counters + 3, J.heads);
     }
 }
@@ -526,18 +415,17 @@ k_direct_scatter_pair(const int64_t* __restrict__ ids_a, int64_t n_a, int64_t ro
     }
 }
 
-template <bool COUNT>
 __global__ void __launch_bounds__(kBT)
 k_bucket_sort_direct(const __grid_constant__ DirectSortJob a, const __grid_constant__ DirectSortJob b) {
     __shared__ uint64_t s[kCap];
     __shared__ int head_cnt, head_base;
-    __shared__ int hist[COUNT ? kCountRows + 1 : 1];
-    __shared__ int scratch[COUNT ? 40 : 1];
+    __shared__ int hist[kCountRows + 1];
+    __shared__ int scratch[40];
     __shared__ int sh[4];
     if (threadIdx.x == 0) head_cnt = 0;
     __syncthreads();
-    if ((int)blockIdx.x < a.grid) direct_sort_job<COUNT>(a, (int)blockIdx.x, s, hist, scratch, &head_cnt, &head_base, sh);
-    else direct_sort_job<COUNT>(b, (int)blockIdx.x - a.grid, s, hist, scratch, &head_cnt, &head_base, sh);
+    if ((int)blockIdx.x < a.grid) direct_sort_job(a, (int)blockIdx.x, s, hist, scratch, &head_cnt, &head_base, sh);
+    else direct_sort_job(b, (int)blockIdx.x - a.grid, s, hist, scratch, &head_cnt, &head_base, sh);
 }
 
 // One table's share of an apply launch: the sorted pairs and row heads of its plan, its contribution sources and
@@ -555,11 +443,11 @@ struct ApplyJob {
     float* M;
     float* V;
     float* dense;
-    int* reset;                  // direct plans: the spill counter, zeroed here for the next step (NULL otherwise)
+    int* reset;                  // the plan's spill counter, zeroed here for the next step
 };
 
 // ---------------------------------------------------------------------------------------------------
-// k_apply_sorted: one lane group per touched row (the head list written by k_bucket_sort): request the weight/state
+// k_apply_sorted: one lane group per touched row (the head list written by k_bucket_sort_direct): request the weight/state
 // rows, sum the row's contributions in ascending position -- the first one is named by the head entry itself, so a
 // row with a single contribution never reads the pair array -- and apply the update.  No barriers, no atomics.
 // Rows with >= kLong contributions (listed by the sort; normally none) are then reduced by whole CTAs: contribution
@@ -666,32 +554,6 @@ static BucketGeom bucket_geom(int64_t n, int64_t n_rows) {
     return g;
 }
 
-struct BucketLayout {
-    size_t count, cursor, off, pairs, tmp, longs, heads, total;
-    int long_cap;
-};
-
-static BucketLayout bucket_layout(int64_t n, int64_t n_rows) {
-    const BucketGeom g = bucket_geom(n, n_rows);
-    BucketLayout L;
-    size_t o = 0;
-    auto take = [&](size_t bytes) {
-        size_t r = o;
-        o += align_up(bytes, 256);
-        return r;
-    };
-    L.count = take((size_t)g.nb * 4 * kPad);
-    L.cursor = take((size_t)g.nb * 4 * kPad);
-    L.off = take((size_t)(g.nb + 4) * 4);
-    L.pairs = take((size_t)n * 8);
-    L.tmp = take((size_t)n * 8);
-    L.long_cap = (int)(n / kLong + 1);
-    L.longs = take((size_t)L.long_cap * 8);
-    L.heads = take((size_t)n * 16);
-    L.total = o;
-    return L;
-}
-
 static BSrc to_bsrc(const b2r_grad_source* s, int d) {
     BSrc r{nullptr, nullptr, nullptr, 0, d, make_fastdiv(1)};
     if (s) {
@@ -705,173 +567,9 @@ static BSrc to_bsrc(const b2r_grad_source* s, int d) {
     return r;
 }
 
-}  // namespace b2r
-
-using namespace b2r;
-
-extern "C" size_t b2r_bucket_workspace_bytes(int64_t n, int64_t n_rows) {
-    if (n <= 0 || n > 0x7fffffff || n_rows <= 0 || n_rows >= 0xffffffffLL) return 0;
-    return bucket_layout(n, n_rows).total;
-}
-
-extern "C" int b2r_bucket_workspace_init(void* ws, size_t ws_bytes, int64_t n, int64_t n_rows, b2r_stream_t stream) {
-    B2R_REQUIRE(ws, B2R_E_BADARG, "b2r_bucket_workspace_init: null pointer");
-    const size_t need = b2r_bucket_workspace_bytes(n, n_rows);
-    B2R_REQUIRE(need != 0 && ws_bytes >= need, B2R_E_WORKSPACE, "b2r_bucket_workspace_init: workspace %zu < %zu", ws_bytes,
-                need);
-    const BucketLayout L = bucket_layout(n, n_rows);
-    // the bucket counters must be zero on entry to b2r_bucket_partition; the scan leaves them zero again
-    B2R_CUDA_OK(cudaMemsetAsync(static_cast<char*>(ws) + L.count, 0, L.cursor - L.count, as_stream(stream)));
-    return 0;
-}
-
-extern "C" int b2r_bucket_partition(const int64_t* ids, int64_t n, int64_t n_rows, int64_t ignore_id, int64_t ignore_n,
-                                    void* ws, size_t ws_bytes, int32_t* err_flag, b2r_stream_t stream) {
-    B2R_REQUIRE(ids && ws, B2R_E_BADARG, "b2r_bucket_partition: null pointer");
-    const size_t need = b2r_bucket_workspace_bytes(n, n_rows);
-    B2R_REQUIRE(need != 0, B2R_E_UNSUPPORTED, "b2r_bucket_partition: n=%lld n_rows=%lld unsupported", (long long)n,
-                (long long)n_rows);
-    B2R_REQUIRE(ws_bytes >= need, B2R_E_WORKSPACE, "b2r_bucket_partition: workspace %zu < %zu", ws_bytes, need);
-    B2R_REQUIRE((reinterpret_cast<uintptr_t>(ws) & 255u) == 0, B2R_E_BADARG, "workspace must be 256-byte aligned");
-    cudaStream_t s = as_stream(stream);
-    const BucketGeom g = bucket_geom(n, n_rows);
-    const BucketLayout L = bucket_layout(n, n_rows);
-    char* base = static_cast<char*>(ws);
-    int* count = reinterpret_cast<int*>(base + L.count);
-    int* cursor = reinterpret_cast<int*>(base + L.cursor);
-    int* off = reinterpret_cast<int*>(base + L.off);
-    uint64_t* pairs = reinterpret_cast<uint64_t*>(base + L.pairs);
-    int grid = (int)((n + kBT * 4 - 1) / (kBT * 4));
-    // next-round sweep knobs (unset = the measured configuration: 8 CTAs per SM for both): how much of each SM the
-    // side-stream plan kernels may occupy next to the HBM-bound kernels of the main stream
-    static const int part_mul = [] { const char* e = getenv("B2R_PART_CAP"); return e && atoi(e) > 0 ? atoi(e) : 8; }();
-    static const int sort_mul = [] { const char* e = getenv("B2R_SORT_CAP"); return e && atoi(e) > 0 ? atoi(e) : 8; }();
-    const int cap = sm_count() * part_mul;
-    if (grid > cap) grid = cap;
-    if (grid < 1) grid = 1;
-    k_bucket_count<<<grid, kBT, 0, s>>>(ids, n, n_rows, g.shift, ignore_id, ignore_n, count, err_flag);
-    B2R_LAUNCH_OK("k_bucket_count");
-    k_bucket_scan<<<1, 1024, 0, s>>>(count, cursor, off, g.nb);
-    B2R_LAUNCH_OK("k_bucket_scan");
-    k_bucket_scatter<<<grid, kBT, 0, s>>>(ids, n, n_rows, g.shift, ignore_id, ignore_n, cursor, pairs);
-    B2R_LAUNCH_OK("k_bucket_scatter");
-    const int sort_cap = sm_count() * sort_mul;
-    // counting sort per bucket is the default (13.3 us vs 20.8 us per launch at config 2, profiles/README r2);
-    // B2R_BUCKET_SORT=bitonic selects the shared-memory bitonic network for A/B runs (same output)
-    static const bool use_count = [] { const char* e = getenv("B2R_BUCKET_SORT"); return !(e && e[0] == 'b'); }();
-    const int sort_grid = g.nb < sort_cap ? g.nb : sort_cap;
-    uint64_t* tmp = reinterpret_cast<uint64_t*>(base + L.tmp);
-    uint2* longs = reinterpret_cast<uint2*>(base + L.longs);
-    uint4* heads = reinterpret_cast<uint4*>(base + L.heads);
-    if (use_count)
-        k_bucket_sort<true><<<sort_grid, kBT, 0, s>>>(pairs, tmp, off, g.nb, off + g.nb + 2, longs, L.long_cap,
-                                                      off + g.nb + 3, heads, g.shift);
-    else
-        k_bucket_sort<false><<<sort_grid, kBT, 0, s>>>(pairs, tmp, off, g.nb, off + g.nb + 2, longs, L.long_cap,
-                                                       off + g.nb + 3, heads, g.shift);
-    B2R_LAUNCH_OK("k_bucket_sort");
-    return 0;
-}
-
-// fills one job from the C-ABI arguments (validated); grid = CTAs it gets
-static int make_job(const b2r_apply_job* j, int d, int mode, const b2r_optim& o, int grid_cap, ApplyJob* out) {
-    B2R_REQUIRE(j->ws && j->s0 && j->s0->src, B2R_E_BADARG, "b2r_bucket_apply: null pointer");
-    B2R_REQUIRE(j->s0->n + (j->s1 ? j->s1->n : 0) == j->n, B2R_E_BADARG,
-                "b2r_bucket_apply: sources cover %lld of %lld positions",
-                (long long)(j->s0->n + (j->s1 ? j->s1->n : 0)), (long long)j->n);
-    if (mode == 1) {
-        B2R_REQUIRE(j->dense, B2R_E_BADARG, "b2r_bucket_apply: mode 1 needs dense");
-    } else {
-        B2R_REQUIRE(j->W, B2R_E_BADARG, "b2r_bucket_apply: mode 2 needs W");
-        B2R_REQUIRE(o.kind != 1 || (j->m && j->v), B2R_E_BADARG, "b2r_bucket_apply: Adam needs m and v");
-        B2R_REQUIRE(o.kind != 2 || j->v, B2R_E_BADARG, "b2r_bucket_apply: Adagrad needs v");
-    }
-    B2R_REQUIRE(b2r_bucket_workspace_bytes(j->n, j->n_rows) != 0, B2R_E_UNSUPPORTED,
-                "b2r_bucket_apply: n=%lld n_rows=%lld unsupported", (long long)j->n, (long long)j->n_rows);
-    const BucketGeom g = bucket_geom(j->n, j->n_rows);
-    const BucketLayout L = bucket_layout(j->n, j->n_rows);
-    const char* base = static_cast<const char*>(j->ws);
-    const int* off = reinterpret_cast<const int*>(base + L.off);
-    out->pairs = reinterpret_cast<const uint64_t*>(base + L.pairs);
-    out->heads = reinterpret_cast<const uint4*>(base + L.heads);
-    out->n_heads = off + g.nb + 3;                   // touched rows, listed by k_bucket_sort
-    out->n_long = off + g.nb + 2;
-    out->longs = reinterpret_cast<const uint2*>(base + L.longs);
-    out->long_cap = L.long_cap;
-    out->s0 = to_bsrc(j->s0, d);
-    out->s1 = to_bsrc(j->s1, d);
-    out->W = j->W; out->M = j->m; out->V = j->v; out->dense = j->dense;
-    out->reset = nullptr;
-    const int gpc = kBT / (d / 4);
-    int64_t need = (j->n + gpc - 1) / gpc;
-    if (need > grid_cap) need = grid_cap;
-    out->grid = (int)(need < 1 ? 1 : need);
-    return 0;
-}
-
-static int apply_pair_common(const b2r_apply_job* ja, const b2r_apply_job* jb, int d, int mode, const b2r_optim* opt,
-                             cudaStream_t s, bool direct);
-
-extern "C" int b2r_bucket_apply_pair(const b2r_apply_job* ja, const b2r_apply_job* jb, int d, int mode,
-                                     const b2r_optim* opt, b2r_stream_t stream) {
-    return apply_pair_common(ja, jb, d, mode, opt, as_stream(stream), false);
-}
-
-namespace b2r {
-int direct_apply_pair(const b2r_apply_job* ja, const b2r_apply_job* jb, int d, int mode, const b2r_optim* opt, cudaStream_t s) {
-    return apply_pair_common(ja, jb, d, mode, opt, s, true);
-}
-}  // namespace b2r
-
-static int make_job_direct(const b2r_apply_job* j, int d, int mode, const b2r_optim& o, int grid_cap, ApplyJob* out);
-
-static int apply_pair_common(const b2r_apply_job* ja, const b2r_apply_job* jb, int d, int mode, const b2r_optim* opt,
-                             cudaStream_t s, bool direct) {
-    B2R_REQUIRE(ja, B2R_E_BADARG, "b2r_bucket_apply: null job");
-    B2R_REQUIRE(d == 32 || d == 64 || d == 128, B2R_E_UNSUPPORTED, "b2r_bucket_apply: d=%d (have 32, 64, 128)", d);
-    B2R_REQUIRE(mode == 1 || mode == 2, B2R_E_BADARG, "b2r_bucket_apply: mode %d (1 = dense +=, 2 = optimizer)", mode);
-    b2r_optim o{};
-    if (mode == 2) {
-        B2R_REQUIRE(opt, B2R_E_BADARG, "b2r_bucket_apply: mode 2 needs opt");
-        o = *opt;
-        B2R_REQUIRE(o.kind >= 0 && o.kind <= 2, B2R_E_BADARG, "b2r_bucket_apply: optimizer kind %d", o.kind);
-    }
-    ApplyJob a{}, b{};
-    const int cap = sm_count() * 16;             // ~2.7 waves of 6 resident CTAs/SM; x12 and x20 measured slower
-    int rc = direct ? make_job_direct(ja, d, mode, o, cap, &a) : make_job(ja, d, mode, o, cap, &a);
-    if (rc != 0) return rc;
-    if (jb != nullptr) {
-        // the second job is the small one by convention; its CTAs come first in the grid so that they are placed at once
-        rc = direct ? make_job_direct(jb, d, mode, o, cap, &b) : make_job(jb, d, mode, o, cap, &b);
-        if (rc != 0) return rc;
-    } else {
-        b = a;
-        b.grid = 0;
-    }
-    const OptK ok = make_optk(o);
-    const int grid = a.grid + b.grid;
-#define B2R_BK(LPR, MODE) k_apply_sorted<LPR, MODE><<<grid, kBT, 0, s>>>(b.grid ? b : a, b.grid ? a : b, ok)
-    if (mode == 1) {
-        if (d == 32) B2R_BK(8, 1); else if (d == 64) B2R_BK(16, 1); else B2R_BK(32, 1);
-    } else {
-        if (d == 32) B2R_BK(8, 2); else if (d == 64) B2R_BK(16, 2); else B2R_BK(32, 2);
-    }
-#undef B2R_BK
-    B2R_LAUNCH_OK("k_apply_sorted");
-    return 0;
-}
-
-extern "C" int b2r_bucket_apply(const void* ws, int64_t n, int64_t n_rows, int d, const b2r_grad_source* s0,
-                                const b2r_grad_source* s1, int mode, float* dense, float* W, float* m, float* v,
-                                const b2r_optim* opt, b2r_stream_t stream) {
-    const b2r_apply_job j{ws, n, n_rows, s0, s1, dense, W, m, v};
-    return b2r_bucket_apply_pair(&j, nullptr, d, mode, opt, stream);
-}
-
 // ---------------------------------------------------------------------------------------------------
 // direct plans (plan_direct.cuh): layout, init, the producer's view, the sort launch, the apply job
 // ---------------------------------------------------------------------------------------------------
-namespace b2r {
 
 struct DirectLayout {
     size_t cursor, region, big, tmp, spill, counters, longs, heads, total;
@@ -1007,15 +705,14 @@ int direct_sort_pair(void* ws_a, int64_t n_a, int64_t rows_a, void* ws_b, int64_
         b = direct_sort_job_of(ws_b, n_b, rows_b, cap);
     }
     // the small plan's CTAs first (they are placed at once), like k_apply_sorted's two jobs
-    if (b.grid) k_bucket_sort_direct<true><<<a.grid + b.grid, kBT, 0, s>>>(b, a);
-    else k_bucket_sort_direct<true><<<a.grid, kBT, 0, s>>>(a, b);
+    if (b.grid) k_bucket_sort_direct<<<a.grid + b.grid, kBT, 0, s>>>(b, a);
+    else k_bucket_sort_direct<<<a.grid, kBT, 0, s>>>(a, b);
     B2R_LAUNCH_OK("k_bucket_sort_direct");
     return 0;
 }
 
-}  // namespace b2r
-
-static int make_job_direct(const b2r_apply_job* j, int d, int mode, const b2r_optim& o, int grid_cap, ApplyJob* out) {
+// fills one job from the C-ABI arguments (validated); grid = CTAs it gets
+static int make_job(const b2r_apply_job* j, int d, int mode, const b2r_optim& o, int grid_cap, ApplyJob* out) {
     B2R_REQUIRE(j->ws && j->s0 && j->s0->src, B2R_E_BADARG, "direct apply: null pointer");
     B2R_REQUIRE(j->s0->n + (j->s1 ? j->s1->n : 0) == j->n, B2R_E_BADARG, "direct apply: sources do not cover the plan");
     if (mode == 1) {
@@ -1046,6 +743,45 @@ static int make_job_direct(const b2r_apply_job* j, int d, int mode, const b2r_op
     out->grid = (int)(need < 1 ? 1 : need);
     return 0;
 }
+
+int direct_apply_pair(const b2r_apply_job* ja, const b2r_apply_job* jb, int d, int mode, const b2r_optim* opt, cudaStream_t s) {
+    B2R_REQUIRE(ja, B2R_E_BADARG, "direct apply: null job");
+    B2R_REQUIRE(d == 32 || d == 64 || d == 128, B2R_E_UNSUPPORTED, "direct apply: d=%d (have 32, 64, 128)", d);
+    B2R_REQUIRE(mode == 1 || mode == 2, B2R_E_BADARG, "direct apply: mode %d (1 = dense +=, 2 = optimizer)", mode);
+    b2r_optim o{};
+    if (mode == 2) {
+        B2R_REQUIRE(opt, B2R_E_BADARG, "direct apply: mode 2 needs opt");
+        o = *opt;
+        B2R_REQUIRE(o.kind >= 0 && o.kind <= 2, B2R_E_BADARG, "direct apply: optimizer kind %d", o.kind);
+    }
+    ApplyJob a{}, b{};
+    const int cap = sm_count() * 16;             // ~2.7 waves of 6 resident CTAs/SM; x12 and x20 measured slower
+    int rc = make_job(ja, d, mode, o, cap, &a);
+    if (rc != 0) return rc;
+    if (jb != nullptr) {
+        // the second job is the small one by convention; its CTAs come first in the grid so that they are placed at once
+        rc = make_job(jb, d, mode, o, cap, &b);
+        if (rc != 0) return rc;
+    } else {
+        b = a;
+        b.grid = 0;
+    }
+    const OptK ok = make_optk(o);
+    const int grid = a.grid + b.grid;
+#define B2R_BK(LPR, MODE) k_apply_sorted<LPR, MODE><<<grid, kBT, 0, s>>>(b.grid ? b : a, b.grid ? a : b, ok)
+    if (mode == 1) {
+        if (d == 32) B2R_BK(8, 1); else if (d == 64) B2R_BK(16, 1); else B2R_BK(32, 1);
+    } else {
+        if (d == 32) B2R_BK(8, 2); else if (d == 64) B2R_BK(16, 2); else B2R_BK(32, 2);
+    }
+#undef B2R_BK
+    B2R_LAUNCH_OK("k_apply_sorted");
+    return 0;
+}
+
+}  // namespace b2r
+
+using namespace b2r;
 
 // ---- C ABI of the direct plans for callers outside a step context (the autograd nodes, the shard owners) -------------
 extern "C" size_t b2r_direct_plan_workspace_bytes(int64_t n, int64_t n_rows) { return direct_workspace_bytes(n, n_rows); }

@@ -74,13 +74,6 @@ SIGNATURES = {
                                     C.POINTER(GradSource), C.POINTER(GradSource), C.c_int, C.c_void_p,
                                     C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
                                     C.POINTER(Optim), C.c_void_p]),
-    "b2r_bucket_workspace_bytes": (C.c_size_t, [C.c_int64, C.c_int64]),
-    "b2r_bucket_workspace_init": (C.c_int, [C.c_void_p, C.c_size_t, C.c_int64, C.c_int64, C.c_void_p]),
-    "b2r_bucket_partition": (C.c_int, [C.c_void_p, C.c_int64, C.c_int64, C.c_int64, C.c_int64, C.c_void_p,
-                                       C.c_size_t, C.c_void_p, C.c_void_p]),
-    "b2r_bucket_apply": (C.c_int, [C.c_void_p, C.c_int64, C.c_int64, C.c_int, C.POINTER(GradSource),
-                                   C.POINTER(GradSource), C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
-                                   C.POINTER(Optim), C.c_void_p]),
     "b2r_direct_plan_workspace_bytes": (C.c_size_t, [C.c_int64, C.c_int64]),
     "b2r_direct_plan_init": (C.c_int, [C.c_void_p, C.c_size_t, C.c_int64, C.c_int64, C.c_void_p]),
     "b2r_direct_plan_build": (C.c_int, [C.c_void_p, C.c_int64, C.c_int64, C.c_int64, C.c_int64, C.c_void_p, C.c_size_t,
@@ -166,7 +159,6 @@ SIGNATURES = {
     "b2r_topk_all_items": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p, C.c_int64, C.c_int, C.c_void_p, C.c_void_p,
                                      C.c_int, C.c_void_p, C.c_void_p, C.c_int64, C.c_int, C.c_void_p, C.c_void_p,
                                      C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p]),
-    "b2r_bucket_apply_pair": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_void_p]),
     "b2r_adam_exact_advance": (C.c_int, [C.c_void_p, C.c_int64, C.c_int64, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p,
                                          C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p]),
     "b2r_sample_negatives": (C.c_int, [C.c_void_p, C.c_int64, C.c_int, C.c_void_p, C.c_void_p, C.c_int64, C.c_int64,

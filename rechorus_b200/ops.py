@@ -597,62 +597,15 @@ class IndexPlan:
         self._apply(W.shape[1], sources, 2, W=W, m=m, v=v, opt=opt)
 
 
-_bucket_ws = {}
-
-
-class BucketPlan:
-    """Bucketed partition of a batch's (row id, position) pairs (b2r_bucket_partition) -- the hot-path sibling of
-    IndexPlan for the dense-add and fused-optimizer outputs (d in {32, 64, 128}).  The workspace is cached per
-    (device, stream, n, n_rows) and reused in stream order."""
-
-    SUPPORTED_D = (32, 64, 128)
-
-    def __init__(self, ids: torch.Tensor, n_rows: int, ignore_id: int = -1, ignore_n: int = 0):
-        _need_cuda(ids)
-        ids = _i64c(ids.reshape(-1), "ids")
-        n = ids.numel()
-        if n == 0:
-            raise ValueError("empty id list")
-        self.n, self.n_rows, self.device = n, int(n_rows), ids.device
-        L = _lib.load()
-        key = (ids.device.index, _stream(), n, self.n_rows)
-        ws = _bucket_ws.get(key)
-        if ws is None:
-            nbytes = L.b2r_bucket_workspace_bytes(n, self.n_rows)
-            if nbytes == 0:
-                raise _lib.B200RecError(f"b2r_bucket_workspace_bytes({n}, {n_rows}) = 0")
-            ws = torch.empty(nbytes, dtype=torch.uint8, device=ids.device)
-            _lib.check(L.b2r_bucket_workspace_init(_p(ws), nbytes, n, self.n_rows, _stream()),
-                       "b2r_bucket_workspace_init")
-            _bucket_ws[key] = ws
-        self.ws = ws
-        self._ids = ids
-        _lib.check(L.b2r_bucket_partition(_p(ids), n, self.n_rows, int(ignore_id), int(ignore_n), _p(ws), ws.numel(),
-                                          _p(err_flag(ids.device)), _stream()), "b2r_bucket_partition")
-
-    def _apply(self, d, sources, mode, dense=None, W=None, m=None, v=None, opt=None):
-        if not 1 <= len(sources) <= 2:
-            raise ValueError("one or two sources")
-        s0 = sources[0].c_struct()
-        s1 = sources[1].c_struct() if len(sources) == 2 else None
-        L = _lib.load()
-        _lib.check(L.b2r_bucket_apply(_p(self.ws), self.n, self.n_rows, d, C.byref(s0),
-                                      C.byref(s1) if s1 is not None else None, mode, _p(dense), _p(W), _p(m), _p(v),
-                                      C.byref(opt) if opt is not None else None, _stream()), "b2r_bucket_apply")
-
-    def add_to_dense(self, dense: torch.Tensor, sources: Sequence[Source]) -> None:
-        self._apply(dense.shape[1], sources, 1, dense=dense)
-
-    def apply_optimizer(self, W: torch.Tensor, m, v, opt: _lib.Optim, sources: Sequence[Source]) -> None:
-        self._apply(W.shape[1], sources, 2, W=W, m=m, v=v, opt=opt)
-
-
 _direct_ws = {}
 
 
 class DirectPlan:
-    """b2r_direct_plan_build / _apply: BucketPlan's job in two launches (scatter into fixed-capacity bucket regions + one
-    sort), same apply kernel.  Workspace cached per (device, stream, n, n_rows) and reused in stream order."""
+    """b2r_direct_plan_build / _apply: bucketed partition of a batch's (row id, position) pairs -- the hot-path sibling of
+    IndexPlan for the dense-add and fused-optimizer outputs (d in {32, 64, 128}): a scatter into fixed-capacity bucket
+    regions and one per-bucket sort.  Workspace cached per (device, stream, n, n_rows) and reused in stream order."""
+
+    SUPPORTED_D = (32, 64, 128)
 
     def __init__(self, ids: torch.Tensor, n_rows: int, ignore_id: int = -1, ignore_n: int = 0):
         _need_cuda(ids)
@@ -696,16 +649,11 @@ class DirectPlan:
         self._apply(W.shape[1], sources, 2, W=W, m=m, v=v, opt=opt)
 
 
-_PLAN_KIND = os.environ.get("B2R_PLAN", "direct")      # direct | bucket (A/B)
-
-
 def make_plan(ids: torch.Tensor, n_rows: int, d: int, ignore_id: int = -1, ignore_n: int = 0):
-    """DirectPlan (two launches) where the bucket kernels exist (d = 32/64/128), IndexPlan (device radix sort) otherwise;
-    B2R_PLAN=bucket selects the four-launch BucketPlan for A/B runs"""
-    if d in BucketPlan.SUPPORTED_D:
-        if _PLAN_KIND == "direct" and DirectPlan.available(ids.numel(), n_rows):
-            return DirectPlan(ids, n_rows, ignore_id, ignore_n)
-        return BucketPlan(ids, n_rows, ignore_id, ignore_n)
+    """DirectPlan (two launches) where its kernels exist (d = 32/64/128) and it can be sized, IndexPlan (device radix
+    sort) otherwise"""
+    if d in DirectPlan.SUPPORTED_D and DirectPlan.available(ids.numel(), n_rows):
+        return DirectPlan(ids, n_rows, ignore_id, ignore_n)
     return IndexPlan(ids, n_rows, ignore_id, ignore_n)
 
 
@@ -881,8 +829,8 @@ def bpr_loss(pred: torch.Tensor) -> torch.Tensor:
 # --------------------------------------------------------------------------------------------------
 
 def bprmf_fused_fwd_bwd(U, uid, I, iid):
-    """b2r_bprmf_fused_fwd_bwd -> (pred [B,C], grad_pred [B,C], row_loss [B], dQ [B,d]); raises when the shape has
-    no fused variant."""
+    """b2r_bprmf_fused_fwd_bwd -> (pred [B,C], grad_pred [B,C], row_loss [B], dQ [B,d]); raises when the shape is
+    outside the streaming kernel's class."""
     _need_cuda(U, I, uid, iid)
     U, I, uid, iid = _f32c(U, "U"), _f32c(I, "I"), _i64c(uid, "uid"), _i64c(iid, "iid")
     B, Cn = iid.shape

@@ -248,9 +248,10 @@ class BPRMFKernels(_KernelModelMixin):
         Needs ``self.optimizer`` to be a ``RowSparseOptimizer``.  ``next_feed_dict`` (optional) is the next
         batch, already on the device: its index plan is prefetched while this step runs.  Returns the loss as a
         device scalar."""
-        if self.emb_size not in (32, 64, 128) or getattr(self.optimizer, "exact_dense", False):
-            # no bucket/fused kernel variant for this width (or the exact dense-Adam mode, which the single-call step
-            # does not implement yet): same step through the autograd nodes
+        if (self.emb_size not in (32, 64, 128) or getattr(self.optimizer, "exact_dense", False)
+                or not ops.DirectPlan.available(feed_dict["item_id"].numel(), self.item_num)):
+            # no plan/apply kernel for this width, the exact dense-Adam mode (which the single-call step does not
+            # implement yet), or a batch too large for the step's index plans: same step through the autograd nodes
             self.optimizer.zero_grad()
             loss = self.loss(self.forward(feed_dict))
             loss.backward()

@@ -338,13 +338,45 @@ def test_train_step_with_prefetched_plan_equals_unprefetched():
             assert torch.equal(pa, pb)
 
 
+def test_train_step_without_direct_plan_takes_autograd_route(monkeypatch):
+    """Batches whose index plans cannot be sized (B*C > 2^30 - 1) train through the autograd nodes and IndexPlan: with
+    DirectPlan reported unavailable, train_step must not enter the single-call step and must leave the same tables as
+    forward -> loss -> backward -> RowSparseOptimizer.step() on the direct plans."""
+    from rechorus_b200 import ops
+    from rechorus_b200.optim import RowSparseOptimizer
+    meta, w, batch, *_ = G.load("bprmf_k9_trained")
+    feed = _cuda_batch(batch, meta["B"])
+    ma, mb = _model(meta, w, "fused"), _model(meta, w, "fused")
+    ma.optimizer = RowSparseOptimizer(ma, "Adam", lr=0.01, l2=1e-5, eps=1e-3)
+    mb.optimizer = RowSparseOptimizer(mb, "Adam", lr=0.01, l2=1e-5, eps=1e-3)
+    losses = []
+    for _ in range(3):
+        ma.optimizer.zero_grad()
+        la = ma.loss(ma(feed))
+        la.backward()
+        ma.optimizer.step()
+        losses.append(float(la))
+
+    def no_step(*a, **k):
+        raise AssertionError("the single-call step was entered")
+
+    monkeypatch.setattr(ops.DirectPlan, "available", staticmethod(lambda n, n_rows: False))
+    monkeypatch.setattr(ops, "bprmf_train_step", no_step)
+    for t in range(3):
+        lb = mb.train_step(feed)
+        assert abs(losses[t] - float(lb)) <= 2e-6
+    for (k, pa), (_, pb) in zip(ma.named_parameters(), mb.named_parameters()):
+        assert (pa - pb).abs().max() <= 1e-6, k
+
+
 @pytest.mark.parametrize("n_rows,n,d,desc", [(1000, 5000, 64, "uniform"), (7, 2560, 64, "7 rows: long rows, one bucket each"),
                                              (3, 9000, 64, "3 rows: oversize buckets (> 2048 pairs of one row)"),
                                              (100000, 3000, 32, "sparse"), (50, 700, 128, "d=128"),
                                              (40, 6000, 64, "hot rows + ignore id")])
-def test_bucket_path_matches_sorted_plan_and_is_reproducible(n_rows, n, d, desc):
-    """b2r_bucket_partition + b2r_bucket_apply (shared-memory sort per bucket) vs the device-radix-sort plan:
-    same dense gradient, same bits on every run, also for hot rows and buckets that overflow shared memory."""
+def test_direct_plan_matches_sorted_plan_and_is_reproducible(n_rows, n, d, desc):
+    """b2r_direct_plan_build + b2r_direct_plan_apply (shared-memory sort per bucket) vs the device-radix-sort plan:
+    same dense gradient, same bits on every run, also for hot rows, long rows (bitonic path), regions that spill and
+    buckets that overflow shared memory (chunk sort + merge)."""
     from rechorus_b200 import lib as L, ops
     g = torch.Generator().manual_seed(n_rows + n)
     ids = torch.randint(0, n_rows, (n,), generator=g)
@@ -360,7 +392,7 @@ def test_bucket_path_matches_sorted_plan_and_is_reproducible(n_rows, n, d, desc)
     outs = []
     for _ in range(2):
         out = torch.zeros(n_rows, d).cuda()
-        ops.BucketPlan(ids.cuda(), n_rows, ign, n if ign >= 0 else 0).add_to_dense(out, [source])
+        ops.DirectPlan(ids.cuda(), n_rows, ign, n if ign >= 0 else 0).add_to_dense(out, [source])
         outs.append(out)
     assert torch.equal(outs[0], outs[1])
     want = torch.zeros(n_rows, d, dtype=torch.float64)
@@ -375,6 +407,6 @@ def test_bucket_path_matches_sorted_plan_and_is_reproducible(n_rows, n, d, desc)
     opt = L.Optim(1, 0.01, 0.9, 0.999, 1e-3, 1e-4, 0.1, 0.001)
     m1, v1, m2, v2 = [torch.zeros_like(W1) for _ in range(4)]
     ops.IndexPlan(ids.cuda(), n_rows, ign, n if ign >= 0 else 0).apply_optimizer(W1, m1, v1, opt, [source])
-    ops.BucketPlan(ids.cuda(), n_rows, ign, n if ign >= 0 else 0).apply_optimizer(W2, m2, v2, opt, [source])
+    ops.DirectPlan(ids.cuda(), n_rows, ign, n if ign >= 0 else 0).apply_optimizer(W2, m2, v2, opt, [source])
     assert (W1 - W2).abs().max() <= 1e-5 and (m1 - m2).abs().max() <= 1e-5 * scale
     ops.check_ids()

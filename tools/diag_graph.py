@@ -22,7 +22,7 @@ except Exception as e:
     import traceback; traceback.print_exc()
     print("FAIL", sys.argv[1:], repr(e)[:300])
 ''' % ROOT
-for env, argv in (({"EAGER_FIRST": "1"}, ["c3"]), ({"EAGER_FIRST": "1"}, ["c4"]), ({"B2R_TC_DW": "0"}, ["c3"]), ({}, ["c3"]), ({}, ["c3", "512"]), ({"B2R_PLAN": "bucket"}, ["c3"]),
+for env, argv in (({"EAGER_FIRST": "1"}, ["c3"]), ({"EAGER_FIRST": "1"}, ["c4"]), ({"B2R_TC_DW": "0"}, ["c3"]), ({}, ["c3"]), ({}, ["c3", "512"]),
                   ({"B2R_TC_DW": "0"}, ["c4"]), ({}, ["c4"]), ({"B2R_SASREC_LIVE": "0", "B2R_TC_DW": "0"}, ["c4"])):
     if os.environ.get("DIAG_ONLY") and "EAGER_FIRST" not in env:
         continue

@@ -24,11 +24,6 @@ for r in rows[1:]:
     except: pass
 for k,v in agg.items(): print(f"  n={len(v):3d} avg={sum(v)/len(v)/1000:8.2f} us  {k}")
 PY
-# how much of each SM the plan kernels may take (default 8 CTAs/SM each): sweep with the best B2R_NEXT setting
-for SC in 2 4 8; do for PC in 4 8; do
-  B2R_SORT_CAP=$SC B2R_PART_CAP=$PC timeout 300 python bench.py --steps 600 --warmup 20 --no_cpu_baseline 2>/dev/null | tail -1 | python -c "
-import sys,json; d=json.loads(sys.stdin.read()); print('sort_cap $SC part_cap $PC: ms %.4f apply %.4f plan %.4f fused %.4f'%(d['ms_per_step'], d['roofline']['kernel_ms'], d['kernels']['plan_items']['ms'], d['kernels']['fused_score_loss_bwd']['ms']))"
-done; done
 # SASRec / NeuMF with every Linear forward on the tcgen05 kernel: parity, step time, tensor-pipe activity
 B2R_TC_LINEAR=1 timeout 600 python -m pytest tests/test_gpu_models.py tests/test_gpu_dense.py -x -q > gpurun_out/n_pytest_tc.log 2>&1; echo "B2R_TC_LINEAR=1 pytest rc=$? $(tail -1 gpurun_out/n_pytest_tc.log)"
 B2R_TC_LINEAR=1 timeout 400 python tools/model_bench.py 2>/dev/null | grep -E '^\{' | cut -c1-200
@@ -36,10 +31,5 @@ timeout 400 ncu --metrics gpu__time_duration.sum,sm__inst_executed_pipe_tensor.s
 # SASRec with the last block computed for one query per sequence (exact; DESIGN.md §8): parity on the fixtures, step time
 B2R_SASREC_LASTQ=1 timeout 600 python -m pytest tests/test_gpu_models.py tests/test_gpu_fullsize.py -x -q > gpurun_out/n_pytest_lastq.log 2>&1; echo "B2R_SASREC_LASTQ=1 pytest rc=$? $(tail -1 gpurun_out/n_pytest_lastq.log)"
 B2R_SASREC_LASTQ=1 timeout 400 python tools/model_bench.py 2>/dev/null | grep -E '^\{' | grep -i sasrec | cut -c1-200
-# where the next batch's plan overlaps: from the step's start (default) or only after the forward kernel
-for PA in 0 1; do
-  B2R_PLAN_AFTER=$PA timeout 300 python bench.py --steps 1000 --warmup 20 --no_cpu_baseline 2>/dev/null | tail -1 | python -c "
-import sys,json; d=json.loads(sys.stdin.read()); print('plan_after $PA: ms %.4f e2e %.4f apply %.4f plan %.4f fused %.4f'%(d['ms_per_step'], d['e2e']['ms_per_step'], d['roofline']['kernel_ms'], d['kernels']['plan_items']['ms'], d['kernels']['fused_score_loss_bwd']['ms']))"
-done
 # Multi-GPU candidate (separate call, charged 2x):  gpurun --gpus 2 -- 'B2R_SHARD_P2P=1 bash tools/gpu_shard.sh 2 nobench'
 # -> the --check line must stay <= 1e-5 / update_ok, then compare the c5 ms_per_step with the NCCL-only run.

@@ -13,9 +13,6 @@ import sys,json
 d=json.loads(sys.stdin.read()); print('c3 ms %.4f e2e %.4f'%(d['ms_per_step'], d['e2e']['ms_per_step']))"
 timeout 300 ncu --metrics gpu__time_duration.sum,sm__inst_executed_pipe_tensor.sum,sm__pipe_tensor_op_umma_cycles_active.avg.pct_of_peak_sustained_active --clock-control none -k regex:k_linear_dw_tc -c 4 --csv --log-file gpurun_out/r2g_dw_tc_pipe.csv python bench.py --workload c4 --steps 3 --warmup 3 --no_cpu_baseline > /dev/null 2>&1; tail -13 gpurun_out/r2g_dw_tc_pipe.csv | cut -d, -f5,13-
 timeout 600 python tools/shard_bench.py --n_items 100000000 --n_users 1000000 --emb 128 --B 4096 --K 255 --steps 20 --warmup 5 2>/dev/null | grep -E "^\{" | cut -c1-160
-B2R_PLAN=bucket timeout 300 python bench.py --steps 300 --warmup 10 --no_cpu_baseline --headline_only 2>/dev/null | tail -1 | python -c "
-import sys,json
-d=json.loads(sys.stdin.read()); print('contract route with bucket plan', d['contract_route']['ms_per_step'])"
 timeout 300 python bench.py --steps 300 --warmup 10 --no_cpu_baseline --headline_only 2>/dev/null | tail -1 | python -c "
 import sys,json
 d=json.loads(sys.stdin.read()); print('contract route with direct plan', d['contract_route']['ms_per_step'], 'c2 ms', d['ms_per_step'])"
