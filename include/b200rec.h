@@ -541,6 +541,10 @@ B2R_API int b2r_bprmf_ctx_destroy(void* ctx);
 /* forget the prefetched plan (call at the start of an epoch and after an aborted one): a prefetched plan is matched to
  * the next batch by its id pointers, which a caching allocator may hand out again for a different batch */
 B2R_API int b2r_bprmf_ctx_reset(void* ctx);
+/* how the context builds the next batch's index plan underneath a step: the plan kernels as persistent grids of at most
+ * `ctas` CTAs (0: grids sized to the work) on a side stream of the highest (high_priority != 0) or the default priority.
+ * The defaults were measured on an H100 at the BASELINE config 2 shape; this entry point is for measuring others. */
+B2R_API int b2r_bprmf_ctx_plan_launch(void* ctx, int ctas, int high_priority);
 B2R_API int b2r_bprmf_train_step(void* ctx, const b2r_bprmf_tables* t, const int64_t* uid, const int64_t* iid,
                          const int64_t* next_uid, const int64_t* next_iid, const b2r_optim* opt,
                          float* loss_out, int32_t* err_flag, b2r_stream_t stream);

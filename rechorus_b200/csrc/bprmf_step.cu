@@ -5,7 +5,11 @@
 //   side :  plan(t+1) for the NEXT batch's ids (or plan(t) itself when nothing was prefetched)
 // The index plan (per-bucket sort of the ids) only depends on the ids, so the context builds it one step ahead on
 // a library-owned non-blocking stream while the HBM-bound kernels of the current step run; joins are event
-// waits, never host synchronisations.  Plans (direct plans, plan_direct.cuh) are double-buffered in the caller-provided
+// waits, never host synchronisations.  The plan has a whole step of slack before the update that reads it, so its
+// kernels run as small persistent grids (kPlanCtas): the forward and optimizer kernels each fill every SM's register
+// file, and every resident plan CTA takes the slot of one of their CTAs.  Sized to the work instead (~1,600 CTAs at
+// config 2, placed first at high priority), the plan pushed part of the forward kernel into a second wave and slowed
+// the optimizer behind it (H100: 0.296 ms per step against 0.265 ms for the two kernels alone).  Plans (direct plans, plan_direct.cuh) are double-buffered in the caller-provided
 // workspace.  d must be 32, 64 or 128 (the widths the plan's apply kernel is built for).  Shapes the streaming forward
 // kernel does not take (C > 1024) run the unfused gather / rowdot / loss / query-backward kernels instead.
 #include "common.cuh"
@@ -48,8 +52,20 @@ static bool step_layout(int B, int C, int d, int64_t n_users, int64_t n_items, S
     return L->dir_i_bytes != 0 && L->dir_u_bytes != 0;
 }
 
+// CTAs of each plan launch of the step (persistent grids; b2r_bprmf_ctx_plan_launch changes them) and the side
+// stream's priority.  Measured on an H100 SXM (700 W) at config 2 with tools/c2_breakdown.py --sweep, ms per step:
+//   CTAs            0 (sized to the work)   66      132     264     528
+//   highest prio    0.284                   0.286   0.287   0.284   0.284
+//   default prio    0.282                   0.356   0.307   0.278   0.282
+// At the default priority the plan's CTAs no longer jump ahead of the forward and optimizer CTAs; 264 (two per SM)
+// keep it fast enough to finish inside its step of slack, fewer starve it.
+constexpr int kPlanCtas = 264;
+constexpr bool kPlanHighPriority = false;
+
 struct StepCtx {
     int B, C, d;
+    int plan_ctas;                    // CTAs per plan launch (0: sized to the work)
+    bool plan_high;                   // side stream at the highest priority
     int64_t n_users, n_items;
     StepLayout L;
     char* ws;
@@ -60,6 +76,14 @@ struct StepCtx {
     const void* pre_iid;
     bool have_pre;
 };
+
+// the plan stream, at the highest or the default priority (kPlanHighPriority)
+static cudaError_t create_side_stream(StepCtx* c) {
+    int prio_lo = 0, prio_hi = 0;
+    cudaError_t e = cudaDeviceGetStreamPriorityRange(&prio_lo, &prio_hi);
+    if (e == cudaSuccess) e = cudaStreamCreateWithPriority(&c->side, cudaStreamNonBlocking, c->plan_high ? prio_hi : prio_lo);
+    return e;
+}
 
 }  // namespace b2r
 
@@ -92,12 +116,9 @@ extern "C" int b2r_bprmf_ctx_create(void** ctx_out, int B, int C, int d, int64_t
     c->slot = 0;
     c->have_pre = false;
     c->pre_uid = c->pre_iid = nullptr;
-    // The plan stream gets the highest priority: its kernels are small, and when the HBM-bound kernels of the main
-    // stream occupy every SM the plan's CTAs must be placed first whenever a slot frees up -- otherwise the plan of
-    // the next batch is starved and the next step's update waits for it (measured: 0.177 vs 0.199 ms per step).
-    int prio_lo = 0, prio_hi = 0;
-    cudaError_t e = cudaDeviceGetStreamPriorityRange(&prio_lo, &prio_hi);
-    if (e == cudaSuccess) e = cudaStreamCreateWithPriority(&c->side, cudaStreamNonBlocking, prio_hi);
+    c->plan_ctas = kPlanCtas;
+    c->plan_high = kPlanHighPriority;
+    cudaError_t e = create_side_stream(c);
     if (e == cudaSuccess) e = cudaEventCreateWithFlags(&c->fork, cudaEventDisableTiming);
     if (e == cudaSuccess) e = cudaEventCreateWithFlags(&c->join[0], cudaEventDisableTiming);
     if (e == cudaSuccess) e = cudaEventCreateWithFlags(&c->join[1], cudaEventDisableTiming);
@@ -141,6 +162,21 @@ extern "C" int b2r_bprmf_ctx_destroy(void* ctx) {
     return 0;
 }
 
+extern "C" int b2r_bprmf_ctx_plan_launch(void* ctx, int ctas, int high_priority) {
+    B2R_REQUIRE(ctx && ctas >= 0, B2R_E_BADARG, "b2r_bprmf_ctx_plan_launch: ctx=%p ctas=%d", ctx, ctas);
+    StepCtx* c = static_cast<StepCtx*>(ctx);
+    c->plan_ctas = ctas;
+    if ((high_priority != 0) != c->plan_high) {
+        // the old stream's work (a prefetched plan) must be complete: the next step joins it through join[], which
+        // records on the new stream from then on
+        B2R_CUDA_OK(cudaStreamSynchronize(c->side));
+        B2R_CUDA_OK(cudaStreamDestroy(c->side));
+        c->plan_high = high_priority != 0;
+        B2R_CUDA_OK(create_side_stream(c));
+    }
+    return 0;
+}
+
 extern "C" int b2r_bprmf_ctx_reset(void* ctx) {
     if (!ctx) return 0;
     StepCtx* c = static_cast<StepCtx*>(ctx);
@@ -154,8 +190,10 @@ static int build_plans(StepCtx* c, int slot, const int64_t* uid, const int64_t* 
     const int64_t n = (int64_t)c->B * c->C;
     profile_begin(B2R_PROF_PLAN_I, c->side);
     int rc = direct_scatter_pair(iid, n, c->n_items, base + c->L.dir_i[slot], uid, c->B, c->n_users,
-                                 base + c->L.dir_u[slot], err_flag, c->side);
-    if (rc == 0) rc = direct_sort_pair(base + c->L.dir_i[slot], n, c->n_items, base + c->L.dir_u[slot], c->B, c->n_users, c->side);
+                                 base + c->L.dir_u[slot], err_flag, c->plan_ctas, c->side);
+    if (rc == 0)
+        rc = direct_sort_pair(base + c->L.dir_i[slot], n, c->n_items, base + c->L.dir_u[slot], c->B, c->n_users,
+                              c->plan_ctas, c->side);
     if (rc != 0) return rc;
     profile_end(B2R_PROF_PLAN_I, c->side);
     B2R_CUDA_OK(cudaEventRecord(c->join[slot], c->side));

@@ -2,8 +2,10 @@
 //   plan side (depends only on the ids; runs on the step context's side stream, one step ahead; plan_direct.cuh):
 //     k_direct_scatter_pair  drops the batch's (row id, position) pairs into fixed-capacity regions of buckets of
 //         2^shift consecutive table rows (~200 pairs each) with one L2 atomic per pair on a line-padded cursor;
-//     k_bucket_sort_direct  one CTA per bucket sorts its pairs by (row, position) in shared memory (counting sort;
-//         bitonic network for rows with many contributions and wide buckets) and writes them back in place.  Buckets
+//     k_bucket_sort_warp  one warp per bucket sorts its pairs by (row, position) (register bitonic network for small
+//         buckets, counting sort in warp-private shared memory otherwise) and writes them back in place;
+//     k_bucket_sort_deferred  one CTA per bucket the warps could not take (spilled, too wide, a row with many
+//         contributions): counting sort or bitonic network in shared memory, chunked merge beyond it.  Buckets
 //         cover ascending disjoint row ranges, so the whole array ends up sorted exactly as a device-wide radix sort
 //         would leave it, at a fraction of the cost; rows with many contributions are listed for the cooperative
 //         reduction; buckets beyond the shared-memory capacity are chunk-sorted and merged.
@@ -324,18 +326,17 @@ __device__ __forceinline__ void sort_one_bucket(uint64_t* g, uint64_t* tg, int c
 }
 
 // ---------------------------------------------------------------------------------------------------
-// k_bucket_sort_direct: one CTA per bucket sorts its (row, position) pairs in place (sort_one_bucket) over plans whose
-// pairs were dropped into fixed-capacity bucket regions by k_direct_scatter_pair (plan_direct.cuh).  A bucket that
-// overflowed its region (skewed ids) first collects its spilled pairs from the spill list into the "big" area behind
-// the regions and is sorted there.  Cursors are left zero for the next step.  Two plans (two tables of one step) ride in
-// one launch.
+// The CTA sort of a direct plan's bucket (sort_one_bucket), for the buckets k_bucket_sort_warp defers.  Pairs were
+// dropped into fixed-capacity bucket regions by k_direct_scatter_pair (plan_direct.cuh).  A bucket that overflowed its
+// region (skewed ids) first collects its spilled pairs from the spill list into the "big" area behind the regions and
+// is sorted there.
 // ---------------------------------------------------------------------------------------------------
 struct DirectSortJob {
-    int nb, cap, shift, grid;
+    int nb, cap, shift;
     int* cursor;
     uint64_t* region;
     uint64_t* spill;
-    int* counters;               // [0] spill count, [1] big cursor, [2] n_long, [3] n_heads
+    int* counters;               // [0] spill count, [1] big cursor, [2] n_long, [3] n_heads, [4] deferred buckets
     int spill_cap;
     uint64_t* big;
     uint64_t* tmp;               // scratch for the merge path, same extent as big
@@ -343,80 +344,279 @@ struct DirectSortJob {
     uint2* longs;
     int long_cap;
     uint4* heads;
+    int2* deferred;              // [nb] (bucket, pair count) the warp sort left to the CTA pass
 };
 
-__device__ __forceinline__ void direct_sort_job(const DirectSortJob& J, int bid, uint64_t* s, int* hist, int* scratch,
-                                                int* head_cnt, int* head_base, int* sh) {
+// one bucket (raw = its cursor's count) by a whole CTA: the region in place, or -- overflow -- region + spilled pairs
+// gathered into the big area
+__device__ __forceinline__ void direct_sort_bucket(const DirectSortJob& J, int b, int raw, uint64_t* s, int* hist,
+                                                   int* scratch, int* head_cnt, int* head_base, int* sh) {
     const int tid = threadIdx.x;
-    for (int b = bid; b < J.nb; b += J.grid) {
-        if (tid == 0) {
-            sh[0] = J.cursor[(int64_t)b * kPadD];
-            J.cursor[(int64_t)b * kPadD] = 0;
-        }
-        __syncthreads();
-        const int raw = sh[0];
-        __syncthreads();
-        if (raw == 0) continue;
-        const uint32_t row0 = (uint32_t)b << J.shift;
-        if (raw <= J.cap) {
-            const int beg = b * J.cap;
-            sort_one_bucket(J.region + (int64_t)beg, J.tmp, raw, beg, row0, J.shift, s, hist, scratch, head_cnt,
-                                   head_base, J.counters + 2, J.longs, J.long_cap, J.counters + 3, J.heads);
-            continue;
-        }
-        // overflow: region (cap pairs) + this bucket's share of the spill list -> contiguous run in the big area
-        const int nsp = min(J.counters[0], J.spill_cap);
-        int mine = 0;
-        for (int i = tid; i < nsp; i += kBT) mine += ((uint32_t)(J.spill[i] >> 32) >> J.shift) == (uint32_t)b ? 1 : 0;
-        if (tid == 0) sh[1] = 0;
-        __syncthreads();
-        if (mine) atomicAdd(&sh[1], mine);
-        __syncthreads();
-        const int total = J.cap + sh[1];
-        if (tid == 0) {
-            sh[2] = atomicAdd(&J.counters[1], total);
-            sh[3] = 0;
-        }
-        __syncthreads();
-        const int base = sh[2];
-        if (base + total > J.big_cap) continue;             // cannot happen (big_cap = 2n); never write out of bounds
-        uint64_t* g = J.big + base;
-        for (int i = tid; i < J.cap; i += kBT) g[i] = J.region[(int64_t)b * J.cap + i];
-        for (int i = tid; i < nsp; i += kBT) {
-            const uint64_t v = J.spill[i];
-            if (((uint32_t)(v >> 32) >> J.shift) == (uint32_t)b) g[J.cap + atomicAdd(&sh[3], 1)] = v;
-        }
-        __syncthreads();
-        // pair indices of the big area continue after the regions: nb * cap + offset
-        sort_one_bucket(g, J.tmp + base, total, J.nb * J.cap + base, row0, J.shift, s, hist, scratch, head_cnt,
+    const uint32_t row0 = (uint32_t)b << J.shift;
+    if (raw <= J.cap) {
+        const int beg = b * J.cap;
+        sort_one_bucket(J.region + (int64_t)beg, J.tmp, raw, beg, row0, J.shift, s, hist, scratch, head_cnt,
                                head_base, J.counters + 2, J.longs, J.long_cap, J.counters + 3, J.heads);
+        return;
+    }
+    // overflow: region (cap pairs) + this bucket's share of the spill list -> contiguous run in the big area
+    const int nsp = min(J.counters[0], J.spill_cap);
+    int mine = 0;
+    for (int i = tid; i < nsp; i += kBT) mine += ((uint32_t)(J.spill[i] >> 32) >> J.shift) == (uint32_t)b ? 1 : 0;
+    if (tid == 0) sh[1] = 0;
+    __syncthreads();
+    if (mine) atomicAdd(&sh[1], mine);
+    __syncthreads();
+    const int total = J.cap + sh[1];
+    if (tid == 0) {
+        sh[2] = atomicAdd(&J.counters[1], total);
+        sh[3] = 0;
+    }
+    __syncthreads();
+    const int base = sh[2];
+    if (base + total > J.big_cap) return;               // cannot happen (big_cap = 2n); never write out of bounds
+    uint64_t* g = J.big + base;
+    for (int i = tid; i < J.cap; i += kBT) g[i] = J.region[(int64_t)b * J.cap + i];
+    for (int i = tid; i < nsp; i += kBT) {
+        const uint64_t v = J.spill[i];
+        if (((uint32_t)(v >> 32) >> J.shift) == (uint32_t)b) g[J.cap + atomicAdd(&sh[3], 1)] = v;
+    }
+    __syncthreads();
+    // pair indices of the big area continue after the regions: nb * cap + offset
+    sort_one_bucket(g, J.tmp + base, total, J.nb * J.cap + base, row0, J.shift, s, hist, scratch, head_cnt,
+                           head_base, J.counters + 2, J.longs, J.long_cap, J.counters + 3, J.heads);
+}
+
+// the pairs of one or two id arrays into their direct plans (one launch; CTAs [0, grid_a) work on a).  Each thread keeps
+// kScatterILP pairs in flight: with the bounded grid of the step context a thread handles many pairs, and one
+// returning L2 atomic at a time would leave the launch latency-bound.
+constexpr int kScatterILP = 4;
+
+__device__ __forceinline__ void scatter_ids(const DirectPlanDev& P, const int64_t* __restrict__ ids, int64_t n,
+                                            int64_t rows, int64_t first, int64_t stride, int32_t* err_flag,
+                                            int64_t ignore_id, int64_t ignore_n) {
+    for (int64_t i0 = first; i0 < n; i0 += stride * kScatterILP) {
+        int64_t id[kScatterILP];
+#pragma unroll
+        for (int u = 0; u < kScatterILP; ++u) {
+            const int64_t i = i0 + u * stride;
+            id[u] = i < n ? ids[i] : -1;
+        }
+#pragma unroll
+        for (int u = 0; u < kScatterILP; ++u) {
+            const int64_t i = i0 + u * stride;
+            if (i >= n || (i < ignore_n && id[u] == ignore_id)) continue;   // padding positions contribute nothing
+            direct_scatter(P, (uint32_t)checked_id(id[u], rows, err_flag), (uint32_t)i);
+        }
     }
 }
 
-// the pairs of one or two id arrays into their direct plans (one launch; CTAs [0, grid_a) work on a)
 __global__ void __launch_bounds__(kBT)
 k_direct_scatter_pair(const int64_t* __restrict__ ids_a, int64_t n_a, int64_t rows_a, const __grid_constant__ DirectPlanDev pa,
                       int grid_a, const int64_t* __restrict__ ids_b, int64_t n_b, int64_t rows_b,
                       const __grid_constant__ DirectPlanDev pb, int32_t* err_flag, int64_t ignore_id, int64_t ignore_n) {
     if (blockIdx.x == 0 && threadIdx.x == 0) {           // counters the following sort accumulates into
-        pa.counters[1] = pa.counters[2] = pa.counters[3] = 0;
-        if (n_b > 0) pb.counters[1] = pb.counters[2] = pb.counters[3] = 0;
+        pa.counters[1] = pa.counters[2] = pa.counters[3] = pa.counters[4] = 0;
+        if (n_b > 0) pb.counters[1] = pb.counters[2] = pb.counters[3] = pb.counters[4] = 0;
     }
     if ((int)blockIdx.x < grid_a) {
-        for (int64_t i = (int64_t)blockIdx.x * kBT + threadIdx.x; i < n_a; i += (int64_t)grid_a * kBT) {
-            const int64_t id = ids_a[i];
-            if (i < ignore_n && id == ignore_id) continue;            // padding positions contribute nothing (plan a only)
-            direct_scatter(pa, (uint32_t)checked_id(id, rows_a, err_flag), (uint32_t)i);
-        }
+        scatter_ids(pa, ids_a, n_a, rows_a, (int64_t)blockIdx.x * kBT + threadIdx.x, (int64_t)grid_a * kBT, err_flag,
+                    ignore_id, ignore_n);                 // the padding rule applies to plan a only
     } else {
         const int gb = (int)gridDim.x - grid_a;
-        for (int64_t i = (int64_t)((int)blockIdx.x - grid_a) * kBT + threadIdx.x; i < n_b; i += (int64_t)gb * kBT)
-            direct_scatter(pb, (uint32_t)checked_id(ids_b[i], rows_b, err_flag), (uint32_t)i);
+        scatter_ids(pb, ids_b, n_b, rows_b, (int64_t)((int)blockIdx.x - grid_a) * kBT + threadIdx.x, (int64_t)gb * kBT,
+                    err_flag, -1, 0);
     }
 }
 
-__global__ void __launch_bounds__(kBT)
-k_bucket_sort_direct(const __grid_constant__ DirectSortJob a, const __grid_constant__ DirectSortJob b) {
+// ---------------------------------------------------------------------------------------------------
+// k_bucket_sort_warp: one warp per bucket, warp-private shared memory, __syncwarp only.  A bucket of a typical batch
+// holds ~200 pairs (items) or ~30 (users): a 256-thread CTA per bucket leaves most of its threads idle and, with 33 KB of
+// shared memory and 64 registers a thread, takes the SM slot of a forward or optimizer CTA.  The warp form keeps the
+// plan's footprint small (kSortWarps warps and kSortWarps * ~8 KB per CTA) so that it can run underneath the step's
+// HBM-bound kernels.  Output is the same as the CTA sort's: the same sorted pair array, the same row heads (the order
+// of the head list differs; nothing depends on it) and the same long rows.
+//   <= kRegSort pairs (any bucket width): bitonic network in registers (two pairs a lane, shuffles);
+//   otherwise, bucket rows <= 2^kWarpShift and pairs <= kWarpCap: counting sort over a warp-private row histogram,
+//       rows with several contributions put in ascending position by insertion sort (at most kRunMax each);
+//   anything else (overflowed into the spill list, a row with > kRunMax contributions, a bucket too wide or too full)
+//       goes on the plan's deferred list for k_bucket_sort_deferred, which runs the CTA sort above.
+// ---------------------------------------------------------------------------------------------------
+constexpr int kSortWarps = 4;            // warps of a k_bucket_sort_warp CTA
+constexpr int kWarpCap = 768;            // pairs a warp sorts in its shared-memory slice (6 KB)
+constexpr int kWarpShift = 9;            // widest bucket a warp's histogram covers: 512 rows (2 KB)
+constexpr int kRegSort = 64;             // pairs sorted in registers
+
+struct WarpSortSmem {
+    uint64_t s[kWarpCap];
+    int hist[(1 << kWarpShift) + 1];
+};
+
+__device__ __forceinline__ uint64_t bitonic_lane(uint64_t v, int i, int j, int k) {
+    const uint64_t p = __shfl_xor_sync(B2R_FULL_MASK, v, j);
+    const bool lower = (i & j) == 0, up = (i & k) == 0;
+    return (lower == up) ? (v < p ? v : p) : (v < p ? p : v);
+}
+
+// cnt <= kRegSort pairs g[0, cnt): sorted in registers (element i in lane i % 32, register i / 32), written back, heads
+// (and long rows, >= kLong contributions) listed with one slot reservation per bucket
+__device__ __forceinline__ void warp_sort_small(const DirectSortJob& J, uint64_t* g, int cnt, int beg) {
+    const int lane = threadIdx.x & 31;
+    uint64_t e0 = lane < cnt ? g[lane] : ~0ull;
+    uint64_t e1 = lane + 32 < cnt ? g[lane + 32] : ~0ull;
+    for (int k = 2; k <= 64; k <<= 1) {
+        for (int j = k >> 1; j > 0; j >>= 1) {
+            if (j == 32) {                               // k == 64: the two registers of a lane, ascending
+                const uint64_t lo = e0 < e1 ? e0 : e1, hi = e0 < e1 ? e1 : e0;
+                e0 = lo;
+                e1 = hi;
+            } else {
+                e0 = bitonic_lane(e0, lane, j, k);
+                e1 = bitonic_lane(e1, lane + 32, j, k);
+            }
+        }
+    }
+    const uint32_t k0 = (uint32_t)(e0 >> 32), k1 = (uint32_t)(e1 >> 32);
+    const uint32_t p0 = __shfl_up_sync(B2R_FULL_MASK, k0, 1), p1 = __shfl_up_sync(B2R_FULL_MASK, k1, 1);
+    const uint32_t last0 = __shfl_sync(B2R_FULL_MASK, k0, 31);
+    const bool h0 = lane < cnt && (lane == 0 || p0 != k0);
+    const bool h1 = lane + 32 < cnt && (lane == 0 ? last0 != k1 : p1 != k1);
+    const uint64_t H = ((uint64_t)__ballot_sync(B2R_FULL_MASK, h1) << 32) | __ballot_sync(B2R_FULL_MASK, h0);
+    int base = 0;
+    if (lane == 0) base = atomicAdd(J.counters + 3, __popcll(H));
+    base = __shfl_sync(B2R_FULL_MASK, base, 0);
+#pragma unroll
+    for (int r = 0; r < 2; ++r) {
+        const int i = lane + 32 * r;
+        const uint64_t v = r ? e1 : e0;
+        if (i < cnt) g[i] = v;
+        if (!(r ? h1 : h0)) continue;
+        const uint64_t after = H & ~((2ull << i) - 1);   // heads behind i (i = 63: none)
+        const int len = (after ? __ffsll((long long)after) - 1 : cnt) - i;
+        const bool is_long = len >= kLong;
+        if (is_long) {
+            const int q = atomicAdd(J.counters + 2, 1);
+            if (q < J.long_cap) J.longs[q] = make_uint2((uint32_t)(beg + i), (uint32_t)len);
+        }
+        J.heads[base + __popcll(H & ((1ull << i) - 1))] =
+            make_uint4((uint32_t)(v >> 32), (uint32_t)v, (uint32_t)(beg + i), is_long ? 0u : (uint32_t)len);
+    }
+}
+
+// counting sort of g[0, cnt) (cnt <= kWarpCap) over rows [row0, row0 + R) (R <= 2^kWarpShift) by one warp.  Returns
+// false, having written nothing, when a row has more than kRunMax contributions.
+__device__ __forceinline__ bool warp_sort_counting(const DirectSortJob& J, uint64_t* g, int cnt, int beg, uint32_t row0,
+                                                   int R, WarpSortSmem& S) {
+    const int lane = threadIdx.x & 31;
+    for (int r = lane; r < R; r += 32) S.hist[r] = 0;
+    __syncwarp();
+    for (int i = lane; i < cnt; i += 32) atomicAdd(&S.hist[(uint32_t)(g[i] >> 32) - row0], 1);
+    __syncwarp();
+    // lane owns rows [lane * RP, (lane + 1) * RP): longest row, touched rows, then an exclusive scan across the warp
+    const int RP = (R + 31) >> 5;
+    int local = 0, mx = 0, rows = 0;
+    for (int x = 0; x < RP; ++x) {
+        const int r = lane * RP + x;
+        if (r < R) {
+            const int c = S.hist[r];
+            local += c;
+            mx = max(mx, c);
+            rows += c > 0 ? 1 : 0;
+        }
+    }
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) mx = max(mx, __shfl_xor_sync(B2R_FULL_MASK, mx, o));
+    int inc = local, rinc = rows;
+#pragma unroll
+    for (int o = 1; o < 32; o <<= 1) {
+        const int y = __shfl_up_sync(B2R_FULL_MASK, inc, o), z = __shfl_up_sync(B2R_FULL_MASK, rinc, o);
+        if (lane >= o) {
+            inc += y;
+            rinc += z;
+        }
+    }
+    if (mx > kRunMax) return false;                      // same value in every lane
+    int run = inc - local;
+    for (int x = 0; x < RP; ++x) {
+        const int r = lane * RP + x;
+        if (r < R) {
+            const int c = S.hist[r];
+            S.hist[r] = run;                             // start of row r; the scatter below moves it to the row's end
+            run += c;
+        }
+    }
+    int base = 0;
+    if (lane == 31) base = atomicAdd(J.counters + 3, rinc);   // rinc of lane 31: the bucket's touched rows
+    base = __shfl_sync(B2R_FULL_MASK, base, 31);
+    __syncwarp();
+    for (int i = lane; i < cnt; i += 32) {
+        const uint64_t v = g[i];
+        S.s[atomicAdd(&S.hist[(uint32_t)(v >> 32) - row0], 1)] = v;
+    }
+    __syncwarp();
+    // row r now spans [hist[r - 1], hist[r]); rows in chunks of 32 (lane = row), heads in ascending row order
+    for (int r0 = 0; r0 < R; r0 += 32) {
+        const int r = r0 + lane;
+        const int a = r < R ? (r ? S.hist[r - 1] : 0) : 0, b = r < R ? S.hist[r] : 0;
+        for (int x = a + 1; x < b; ++x) {                // insertion sort of the row's run by (row, position)
+            const uint64_t val = S.s[x];
+            int y = x - 1;
+            while (y >= a && S.s[y] > val) {
+                S.s[y + 1] = S.s[y];
+                --y;
+            }
+            S.s[y + 1] = val;
+        }
+        const unsigned m = __ballot_sync(B2R_FULL_MASK, b > a);
+        if (b > a)
+            J.heads[base + __popc(m & ((1u << lane) - 1))] =
+                make_uint4(row0 + (uint32_t)r, (uint32_t)S.s[a], (uint32_t)(beg + a), (uint32_t)(b - a));
+        base += __popc(m);
+    }
+    __syncwarp();
+    for (int i = lane; i < cnt; i += 32) g[i] = S.s[i];
+    __syncwarp();
+    return true;
+}
+
+// warps of the launch walk the buckets of b (the small plan) and then a, kSortWarps * gridDim.x at a time.  At most 32
+// registers a thread (16 CTAs' worth of an SM's register file): a resident sort CTA costs an SM a few percent of its
+// registers and ~33 KB of shared memory.
+__global__ void __launch_bounds__(kSortWarps * 32, 16)
+k_bucket_sort_warp(const __grid_constant__ DirectSortJob a, const __grid_constant__ DirectSortJob b) {
+    __shared__ WarpSortSmem smem[kSortWarps];
+    const int lane = threadIdx.x & 31, wl = threadIdx.x >> 5;
+    WarpSortSmem& S = smem[wl];
+    const int total = a.nb + b.nb;
+    for (int q = (int)blockIdx.x * kSortWarps + wl; q < total; q += (int)gridDim.x * kSortWarps) {
+        const bool in_b = q < b.nb;
+        const DirectSortJob& J = in_b ? b : a;
+        const int bk = in_b ? q : q - b.nb;
+        int raw = 0;
+        if (lane == 0) {
+            raw = J.cursor[(int64_t)bk * kPadD];
+            if (raw) J.cursor[(int64_t)bk * kPadD] = 0;  // left zero for the next plan
+        }
+        raw = __shfl_sync(B2R_FULL_MASK, raw, 0);
+        if (raw == 0) continue;
+        const int beg = bk * J.cap;
+        if (raw <= kRegSort) {                           // cap >= 128: never an overflowed bucket
+            warp_sort_small(J, J.region + beg, raw, beg);
+            continue;
+        }
+        if (raw <= J.cap && raw <= kWarpCap && J.shift <= kWarpShift &&
+            warp_sort_counting(J, J.region + beg, raw, beg, (uint32_t)bk << J.shift, 1 << J.shift, S))
+            continue;
+        if (lane == 0) J.deferred[atomicAdd(J.counters + 4, 1)] = make_int2(bk, raw);
+    }
+}
+
+// the buckets the warp sort deferred, one CTA each; exits at once when there are none (the usual case).  all_buckets:
+// every bucket of both plans instead, straight from the cursors (plans of a few buckets: one launch, no warp pass).
+__global__ void __maxnreg__(64)
+k_bucket_sort_deferred(const __grid_constant__ DirectSortJob a, const __grid_constant__ DirectSortJob b, int all_buckets) {
+    const int nda = all_buckets ? a.nb : a.counters[4], ndb = all_buckets ? b.nb : b.nb ? b.counters[4] : 0;
+    if (nda + ndb == 0) return;
     __shared__ uint64_t s[kCap];
     __shared__ int head_cnt, head_base;
     __shared__ int hist[kCountRows + 1];
@@ -424,8 +624,27 @@ k_bucket_sort_direct(const __grid_constant__ DirectSortJob a, const __grid_const
     __shared__ int sh[4];
     if (threadIdx.x == 0) head_cnt = 0;
     __syncthreads();
-    if ((int)blockIdx.x < a.grid) direct_sort_job(a, (int)blockIdx.x, s, hist, scratch, &head_cnt, &head_base, sh);
-    else direct_sort_job(b, (int)blockIdx.x - a.grid, s, hist, scratch, &head_cnt, &head_base, sh);
+    for (int q = (int)blockIdx.x; q < nda + ndb; q += (int)gridDim.x) {
+        if (all_buckets) {
+            const DirectSortJob& J = q < nda ? a : b;
+            const int bk = q < nda ? q : q - nda;
+            if (threadIdx.x == 0) {
+                sh[0] = J.cursor[(int64_t)bk * kPadD];
+                J.cursor[(int64_t)bk * kPadD] = 0;
+            }
+            __syncthreads();
+            const int raw = sh[0];
+            __syncthreads();
+            if (raw != 0) direct_sort_bucket(J, bk, raw, s, hist, scratch, &head_cnt, &head_base, sh);
+        } else if (q < nda) {
+            const int2 e = a.deferred[q];
+            direct_sort_bucket(a, e.x, e.y, s, hist, scratch, &head_cnt, &head_base, sh);
+        } else {
+            const int2 e = b.deferred[q - nda];
+            direct_sort_bucket(b, e.x, e.y, s, hist, scratch, &head_cnt, &head_base, sh);
+        }
+        __syncthreads();
+    }
 }
 
 // One table's share of an apply launch: the sorted pairs and row heads of its plan, its contribution sources and
@@ -447,7 +666,7 @@ struct ApplyJob {
 };
 
 // ---------------------------------------------------------------------------------------------------
-// k_apply_sorted: one lane group per touched row (the head list written by k_bucket_sort_direct): request the weight/state
+// k_apply_sorted: one lane group per touched row (the head list written by the plan's sort): request the weight/state
 // rows, sum the row's contributions in ascending position -- the first one is named by the head entry itself, so a
 // row with a single contribution never reads the pair array -- and apply the update.  No barriers, no atomics.
 // Rows with >= kLong contributions (listed by the sort; normally none) are then reduced by whole CTAs: contribution
@@ -572,7 +791,7 @@ static BSrc to_bsrc(const b2r_grad_source* s, int d) {
 // ---------------------------------------------------------------------------------------------------
 
 struct DirectLayout {
-    size_t cursor, region, big, tmp, spill, counters, longs, heads, total;
+    size_t cursor, region, big, tmp, spill, counters, longs, heads, deferred, total;
     int nb, shift, cap, big_cap, spill_cap, long_cap;
 };
 
@@ -604,6 +823,7 @@ static DirectLayout direct_layout(int64_t n, int64_t n_rows) {
     L.spill = take((size_t)L.spill_cap * 8);
     L.longs = take((size_t)L.long_cap * 8);
     L.heads = take((size_t)n * 16);
+    L.deferred = take((size_t)L.nb * 8);
     L.total = o;
     return L;
 }
@@ -642,12 +862,11 @@ DirectPlanDev direct_plan_dev(void* ws, int64_t n, int64_t n_rows) {
     return P;
 }
 
-static DirectSortJob direct_sort_job_of(void* ws, int64_t n, int64_t n_rows, int grid_cap) {
+static DirectSortJob direct_sort_job_of(void* ws, int64_t n, int64_t n_rows) {
     const DirectLayout L = direct_layout(n, n_rows);
     char* base = static_cast<char*>(ws);
     DirectSortJob J;
     J.nb = L.nb; J.cap = L.cap; J.shift = L.shift;
-    J.grid = L.nb < grid_cap ? L.nb : grid_cap;
     J.cursor = reinterpret_cast<int*>(base + L.cursor);
     J.region = reinterpret_cast<uint64_t*>(base + L.region);
     J.spill = reinterpret_cast<uint64_t*>(base + L.spill);
@@ -659,21 +878,22 @@ static DirectSortJob direct_sort_job_of(void* ws, int64_t n, int64_t n_rows, int
     J.longs = reinterpret_cast<uint2*>(base + L.longs);
     J.long_cap = L.long_cap;
     J.heads = reinterpret_cast<uint4*>(base + L.heads);
+    J.deferred = reinterpret_cast<int2*>(base + L.deferred);
     return J;
 }
 
 static int direct_scatter_pair_ex(const int64_t* ids_a, int64_t n_a, int64_t rows_a, void* ws_a, const int64_t* ids_b,
                                   int64_t n_b, int64_t rows_b, void* ws_b, int32_t* err_flag, int64_t ignore_id,
-                                  int64_t ignore_n, cudaStream_t s);
+                                  int64_t ignore_n, int ctas, cudaStream_t s);
 
 int direct_scatter_pair(const int64_t* ids_a, int64_t n_a, int64_t rows_a, void* ws_a, const int64_t* ids_b, int64_t n_b,
-                        int64_t rows_b, void* ws_b, int32_t* err_flag, cudaStream_t s) {
-    return direct_scatter_pair_ex(ids_a, n_a, rows_a, ws_a, ids_b, n_b, rows_b, ws_b, err_flag, -1, 0, s);
+                        int64_t rows_b, void* ws_b, int32_t* err_flag, int ctas, cudaStream_t s) {
+    return direct_scatter_pair_ex(ids_a, n_a, rows_a, ws_a, ids_b, n_b, rows_b, ws_b, err_flag, -1, 0, ctas, s);
 }
 
 static int direct_scatter_pair_ex(const int64_t* ids_a, int64_t n_a, int64_t rows_a, void* ws_a, const int64_t* ids_b,
                                   int64_t n_b, int64_t rows_b, void* ws_b, int32_t* err_flag, int64_t ignore_id,
-                                  int64_t ignore_n, cudaStream_t s) {
+                                  int64_t ignore_n, int ctas, cudaStream_t s) {
     B2R_REQUIRE(ids_a && ws_a && direct_ok(n_a, rows_a), B2R_E_BADARG, "direct_scatter_pair: bad plan a");
     const DirectPlanDev pa = direct_plan_dev(ws_a, n_a, rows_a);
     DirectPlanDev pb = pa;
@@ -689,25 +909,54 @@ static int direct_scatter_pair_ex(const int64_t* ids_a, int64_t n_a, int64_t row
     if (ga < 1) ga = 1;
     int gb = nb > 0 ? (int)((nb + kBT * 4 - 1) / (kBT * 4)) : 0;
     if (gb > cap) gb = cap;
+    if (ctas > 0 && ga + gb > ctas) {                    // bounded: split the CTAs in proportion to the pairs
+        const int want_b = gb;
+        gb = nb > 0 ? (int)((int64_t)ctas * nb / (n_a + nb)) : 0;
+        if (want_b > 0 && gb < 1) gb = 1;
+        ga = ctas - gb;
+        if (ga < 1) ga = 1;
+    }
     k_direct_scatter_pair<<<ga + gb, kBT, 0, s>>>(ids_a, n_a, rows_a, pa, ga, ids_b, nb, rows_b, pb, err_flag, ignore_id,
                                                   ignore_n);
     B2R_LAUNCH_OK("k_direct_scatter_pair");
     return 0;
 }
 
-int direct_sort_pair(void* ws_a, int64_t n_a, int64_t rows_a, void* ws_b, int64_t n_b, int64_t rows_b, cudaStream_t s) {
+// the warp sort takes (nearly) every bucket of a typical batch of this plan: its buckets fit a warp's histogram and
+// slice, or they hold so few pairs on average (<= 3/4 of kRegSort) that the register sort takes all but a vanishing tail
+static bool warp_takes_most(const DirectSortJob& J, int64_t n) {
+    return (J.shift <= kWarpShift && J.cap <= kWarpCap) || n <= (int64_t)J.nb * (kRegSort * 3 / 4);
+}
+
+int direct_sort_pair(void* ws_a, int64_t n_a, int64_t rows_a, void* ws_b, int64_t n_b, int64_t rows_b, int ctas,
+                     cudaStream_t s) {
     B2R_REQUIRE(ws_a && direct_ok(n_a, rows_a), B2R_E_BADARG, "direct_sort_pair: bad plan a");
-    const int cap = sm_count() * 8;
-    DirectSortJob a = direct_sort_job_of(ws_a, n_a, rows_a, cap), b = a;
-    b.grid = 0;
+    DirectSortJob a = direct_sort_job_of(ws_a, n_a, rows_a), b = a;
+    b.nb = 0;
     if (ws_b != nullptr) {
         B2R_REQUIRE(direct_ok(n_b, rows_b), B2R_E_BADARG, "direct_sort_pair: bad plan b");
-        b = direct_sort_job_of(ws_b, n_b, rows_b, cap);
+        b = direct_sort_job_of(ws_b, n_b, rows_b);
     }
-    // the small plan's CTAs first (they are placed at once), like k_apply_sorted's two jobs
-    if (b.grid) k_bucket_sort_direct<<<a.grid + b.grid, kBT, 0, s>>>(b, a);
-    else k_bucket_sort_direct<<<a.grid, kBT, 0, s>>>(a, b);
-    B2R_LAUNCH_OK("k_bucket_sort_direct");
+    if (a.nb + b.nb <= sm_count()) {
+        // a few buckets (small batches, e.g. BASELINE config 1): one CTA each in one launch -- the warp pass would only
+        // add a launch to a step bound by launch latency
+        k_bucket_sort_deferred<<<a.nb + b.nb, kBT, 0, s>>>(a, b, 1);
+        B2R_LAUNCH_OK("k_bucket_sort_deferred");
+        return 0;
+    }
+    // a warp per bucket (ctas = 0: as many warps as buckets); the buckets of the small plan come first
+    int grid = (a.nb + b.nb + kSortWarps - 1) / kSortWarps;
+    if (ctas > 0 && grid > ctas) grid = ctas;
+    k_bucket_sort_warp<<<grid, kSortWarps * 32, 0, s>>>(a, b);
+    B2R_LAUNCH_OK("k_bucket_sort_warp");
+    // deferred buckets: normally none, and the launch's CTAs exit at once.  Plans whose buckets are mostly beyond the
+    // warp sort (too wide and too full, e.g. 8,192-row buckets of ~340 pairs) defer nearly all of them: those get a grid
+    // sized to their buckets, as the CTA sort always had.
+    int dgrid = sm_count();
+    if (ctas > 0 && dgrid > ctas) dgrid = ctas;
+    if (!warp_takes_most(a, n_a) || (b.nb && !warp_takes_most(b, n_b))) dgrid = min(a.nb + b.nb, sm_count() * 8);
+    k_bucket_sort_deferred<<<dgrid, kBT, 0, s>>>(a, b, 0);
+    B2R_LAUNCH_OK("k_bucket_sort_deferred");
     return 0;
 }
 
@@ -798,12 +1047,12 @@ extern "C" int b2r_direct_plan_build(const int64_t* ids, int64_t n, int64_t n_ro
                 (long long)n_rows);
     B2R_REQUIRE(ws_bytes >= need, B2R_E_WORKSPACE, "b2r_direct_plan_build: workspace %zu < %zu", ws_bytes, need);
     cudaStream_t s = as_stream(stream);
-    // a plan that was built but never applied leaves its spill counter set: clear the four counters here
+    // a plan that was built but never applied leaves its spill counter set: clear the five counters here
     const DirectPlanDev P = direct_plan_dev(ws, n, n_rows);
-    B2R_CUDA_OK(cudaMemsetAsync(P.counters, 0, 16, s));
-    int rc = direct_scatter_pair_ex(ids, n, n_rows, ws, nullptr, 0, 0, nullptr, err_flag, ignore_id, ignore_n, s);
+    B2R_CUDA_OK(cudaMemsetAsync(P.counters, 0, 20, s));
+    int rc = direct_scatter_pair_ex(ids, n, n_rows, ws, nullptr, 0, 0, nullptr, err_flag, ignore_id, ignore_n, 0, s);
     if (rc != 0) return rc;
-    return direct_sort_pair(ws, n, n_rows, nullptr, 0, 0, s);
+    return direct_sort_pair(ws, n, n_rows, nullptr, 0, 0, 0, s);
 }
 
 extern "C" int b2r_direct_plan_apply(const void* ws, int64_t n, int64_t n_rows, int d, const b2r_grad_source* s0,

@@ -1,8 +1,9 @@
 // plan_direct.cuh -- the "direct" index plan of a table's row-sparse update (bucket.cu; used by the step context of
 // bprmf_step.cu and by the b2r_direct_plan_* entry points).  One scatter launch drops each (row, position) pair of the
 // batch into the bucket of its row range: fixed-capacity bucket regions, one L2 atomic per pair on a line-padded cursor,
-// pairs beyond a region's capacity (skewed batches) into a spill list.  One sort launch then orders every bucket
-// (k_bucket_sort_direct) and lists the row heads for k_apply_sorted.  Both launches can carry two tables.
+// pairs beyond a region's capacity (skewed batches) into a spill list.  The sort then orders every bucket -- a warp per
+// bucket (k_bucket_sort_warp), a CTA for the few it defers (k_bucket_sort_deferred) -- and lists the row heads for
+// k_apply_sorted.  Every launch can carry two tables.
 #pragma once
 #include "common.cuh"
 
@@ -14,7 +15,8 @@ struct DirectPlanDev {                    // what the scatter kernel needs
     int* cursor;                          // [nb * kPadD]
     uint64_t* region;                     // [nb][cap] pairs (row << 32 | position)
     uint64_t* spill;                      // [spill_cap] pairs that did not fit their region
-    int* counters;                        // [0] spill count, [1] big-area cursor, [2] long rows, [3] row heads
+    int* counters;                        // [0] spill count, [1] big-area cursor, [2] long rows, [3] row heads,
+                                          // [4] buckets deferred to the CTA sort
     int cap, shift, spill_cap;
 };
 
@@ -34,11 +36,15 @@ size_t direct_workspace_bytes(int64_t n, int64_t n_rows);
 int direct_workspace_init(void* ws, size_t ws_bytes, int64_t n, int64_t n_rows, cudaStream_t s);
 DirectPlanDev direct_plan_dev(void* ws, int64_t n, int64_t n_rows);
 // drop the pairs of one or two id arrays into their plans in ONE launch (the step context: the NEXT batch's ids on its
-// side stream)
+// side stream).  ctas > 0 bounds the launch to that many CTAs (a persistent grid looping over the pairs); 0 sizes it to
+// the work.
 int direct_scatter_pair(const int64_t* ids_a, int64_t n_a, int64_t rows_a, void* ws_a, const int64_t* ids_b, int64_t n_b,
-                        int64_t rows_b, void* ws_b, int32_t* err_flag, cudaStream_t s);
-// sort every bucket of one or two plans (b may be NULL) in ONE launch and list their row heads
-int direct_sort_pair(void* ws_a, int64_t n_a, int64_t rows_a, void* ws_b, int64_t n_b, int64_t rows_b, cudaStream_t s);
+                        int64_t rows_b, void* ws_b, int32_t* err_flag, int ctas, cudaStream_t s);
+// sort every bucket of one or two plans (b may be NULL) and list their row heads: a warp per bucket in one launch, then
+// one CTA per bucket the warps could not take in a second launch (empty for a typical batch); plans with at most one
+// bucket per SM take the CTA sort in a single launch.  ctas > 0 bounds the launches as above.
+int direct_sort_pair(void* ws_a, int64_t n_a, int64_t rows_a, void* ws_b, int64_t n_b, int64_t rows_b, int ctas,
+                     cudaStream_t s);
 // One table's share of an apply launch: its plan, the contribution sources, and the arrays to update (mode 1: dense +=;
 // mode 2: W and the optimizer state m, v).
 struct b2r_apply_job {

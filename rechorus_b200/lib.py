@@ -197,6 +197,7 @@ SIGNATURES = {
                                        C.c_void_p, C.c_size_t]),
     "b2r_bprmf_ctx_destroy": (C.c_int, [C.c_void_p]),
     "b2r_bprmf_ctx_reset": (C.c_int, [C.c_void_p]),
+    "b2r_bprmf_ctx_plan_launch": (C.c_int, [C.c_void_p, C.c_int, C.c_int]),
     "b2r_bprmf_train_step": (C.c_int, [C.c_void_p, C.POINTER(BprmfTables), C.c_void_p, C.c_void_p, C.c_void_p,
                                        C.c_void_p, C.POINTER(Optim), C.c_void_p, C.c_void_p, C.c_void_p]),
 }
