@@ -25,7 +25,7 @@
 extern "C" {
 #endif
 
-#define B2R_VERSION 102          /* major*10000 + minor*100 + patch */
+#define B2R_VERSION 103          /* major*10000 + minor*100 + patch */
 
 #define B2R_E_BADARG   (-1)      /* null pointer, d % 4 != 0, negative size ... */
 #define B2R_E_WORKSPACE (-2)     /* workspace too small */
@@ -41,8 +41,6 @@ typedef void* b2r_stream_t;      /* cudaStream_t */
 
 B2R_API int         b2r_version(void);
 B2R_API const char* b2r_last_error(void);
-/* sm count / compute capability of the current device (132 / 9.0 on an H100 SXM) */
-B2R_API int         b2r_device_info(int* sm_count, int* cc_major, int* cc_minor);
 
 /* Measurement hooks for bench.py (no effect on results):
  *  - b2r_launch_count(): kernels launched by this library so far (a CUB device-wide call counts as one);
@@ -88,8 +86,7 @@ B2R_API int b2r_gather_rows_strided(const float* T, const int64_t* ids, int64_t 
 B2R_API int b2r_pairdot_fwd(const float* Q, const int64_t* qidx, int64_t n_q, const float* T, const int64_t* rows,
                     int64_t n_t, float* out, int64_t n, int d, int32_t* err_flag, b2r_stream_t stream);
 
-/* Groundwork, opt-in (B2R_SHARD_P2P=1), not used by the default paths of this round: b2r_pairdot_fwd whose result for
- * pair e is stored at out_tab[e / seg][e % seg] -- out_tab is a DEVICE array of n / seg pointers, typically the
+/* The scoring hop of the default config-5 exchange (exchange="p2p"): b2r_pairdot_fwd whose result for pair e is stored at out_tab[e / seg][e % seg] -- out_tab is a DEVICE array of n / seg pointers, typically the
  * peer-mapped receive buffers of the ranks the pairs came from (torch.distributed._symmetric_memory), so the scores
  * reach their requesters by NVLink stores from inside the kernel instead of an all-to-all. */
 B2R_API int b2r_pairdot_fwd_p2p(const float* Q, const int64_t* qidx, int64_t n_q, const float* T, const int64_t* rows,
@@ -120,12 +117,9 @@ B2R_API int b2r_bpr_loss(const float* pred, float* loss_out, float* grad_pred, f
  *        seg_start[n] int32 (index into sorted_* where unique row u starts), n_uniq (device int32)
  * ---------------------------------------------------------------------------------------------- */
 B2R_API size_t b2r_plan_workspace_bytes(int64_t n, int64_t n_rows);
-B2R_API int b2r_plan_build(const int64_t* ids, int64_t n, int64_t n_rows,
-                   uint32_t* sorted_key, uint32_t* sorted_pos, int32_t* seg_start, int32_t* n_uniq,
-                   void* ws, size_t ws_bytes, int32_t* err_flag, b2r_stream_t stream);
-/* same, but positions p < ignore_n whose id equals ignore_id are dropped from the gradient (they get the
- * sentinel key n_rows, which b2r_segment_apply skips): the right-padding of SASRec histories, whose
- * gradient is exactly zero in the reference (SASRec.py:74 masks them) */
+/* positions p < ignore_n whose id equals ignore_id are dropped from the gradient (they get the sentinel key n_rows,
+ * which b2r_segment_apply skips): the right-padding of SASRec histories, whose gradient is exactly zero in the
+ * reference (SASRec.py:74 masks them).  ignore_n = 0 keeps every position. */
 B2R_API int b2r_plan_build_ex(const int64_t* ids, int64_t n, int64_t n_rows, int64_t ignore_id, int64_t ignore_n,
                       uint32_t* sorted_key, uint32_t* sorted_pos, int32_t* seg_start, int32_t* n_uniq,
                       void* ws, size_t ws_bytes, int32_t* err_flag, b2r_stream_t stream);
@@ -194,10 +188,6 @@ B2R_API int b2r_direct_plan_build(const int64_t* ids, int64_t n, int64_t n_rows,
 B2R_API int b2r_direct_plan_apply(const void* ws, int64_t n, int64_t n_rows, int d, const b2r_grad_source* s0,
                                   const b2r_grad_source* s1, int mode, float* dense, float* W, float* m, float* v,
                                   const b2r_optim* opt, b2r_stream_t stream);
-
-/* Fast, order-nondeterministic alternative to plan+segment for mode 1 (dense += via red.global.add.v4.f32) */
-B2R_API int b2r_scatter_add_atomic(const int64_t* ids, int64_t n_rows, const b2r_grad_source* s, int d,
-                           float* dense, int32_t* err_flag, b2r_stream_t stream);
 
 /* Dense optimizer step over a whole parameter tensor (exact torch.optim semantics; used for the small dense
  * parameters of NeuMF/SASRec and for the exact-reference dense-Adam mode of the embedding tables). */
@@ -307,9 +297,9 @@ B2R_API int b2r_add_layernorm_bwd_dropout(const float* dy, const float* x, const
  * SASRec sequence kernels (models/sequential/SASRec.py:51-86, utils/layers.py:34-63).
  *   embed_history : x[b,t,:] = I[hist[b,t]] + P[(len[b]-t) * (hist[b,t] > 0)]; pos_out (optional) gets the
  *                   position index used per element                                    (SASRec.py:58-66)
- *   attention_fwd : causal multi-head attention, heads = contiguous d/H chunks, scores / sqrt(d/H),
+ *   attention_fwd_live : causal multi-head attention, heads = contiguous d/H chunks, scores / sqrt(d/H),
  *                   softmax over keys j <= i, no output projection; q,k,v rows at ld stride (layers.py:52-63)
- *   attention_bwd : recomputes the probabilities; writes dq, dk, dv rows at ldg stride.  L <= 128.
+ *   attention_bwd_live : recomputes the probabilities; writes dq, dk, dv rows at ldg stride.  L <= 128.
  *   select_last   : h[b] = y[b, len[b]-1] * (hist[b, len[b]-1] > 0)                    (SASRec.py:74-76)
  *   small_table_grad : dense gradient of a small table shared by many positions (the position table):
  *                   dense_out[id] = sum_{r: ids[r]=id} src[r], fixed order, no atomics.
@@ -317,11 +307,7 @@ B2R_API int b2r_add_layernorm_bwd_dropout(const float* dy, const float* x, const
 B2R_API int b2r_embed_history(const float* I, int64_t n_items, const float* P, int64_t n_pos, const int64_t* hist,
                       const int64_t* lengths, float* x, int64_t* pos_out, int B, int L, int d,
                       int32_t* err_flag, b2r_stream_t stream);
-B2R_API int b2r_attention_fwd(const float* q, const float* k, const float* v, int ld, float* ctx, int B, int L, int d,
-                      int H, b2r_stream_t stream);
-B2R_API int b2r_attention_bwd(const float* q, const float* k, const float* v, int ld, const float* dctx, float* dq,
-                      float* dk, float* dv, int ldg, int B, int L, int d, int H, b2r_stream_t stream);
-/* The same with dead rows skipped: live[b] (int64, NULL = L) is the number of leading positions of sequence b whose
+/* Attention with dead rows skipped: live[b] (int64, NULL = L) is the number of leading positions of sequence b whose
  * output anything downstream reads -- SASRec uses position len-1 only (SASRec.py:74-81) and attention is causal, so the
  * positions >= len are exact dead work (forward and backward).  Dead rows of ctx / dq / dk / dv are written as zeros. */
 B2R_API int b2r_attention_fwd_live(const float* q, const float* k, const float* v, int ld, const int64_t* live, float* ctx,
@@ -344,8 +330,8 @@ B2R_API int b2r_attention_bwd_rt(const float* q, const float* k, const float* v,
  * sequence -- the query at position t* = clamp(lengths[b]-1, 0, L-1), the only position of SASRec's last block whose
  * output is used (models/sequential/SASRec.py:74-81) -- against keys/values 0..t* (the causal row of
  * utils/layers.py:52-63).  q_last, ctx_last, dq_last are [B, d]; k, v, dk, dv are [B, L, d] rows with leading
- * dimension ld / ldg; prob [B, H, L] keeps the softmax row for the backward.  Identical results to b2r_attention_fwd/
- * bwd restricted to that query; rows of dk, dv beyond t* are written as zeros. */
+ * dimension ld / ldg; prob [B, H, L] keeps the softmax row for the backward.  Identical results to
+ * b2r_attention_fwd/bwd_live restricted to that query; rows of dk, dv beyond t* are written as zeros. */
 B2R_API int b2r_attention_last_fwd(const float* q_last, const float* k, const float* v, int ld, const int64_t* lengths,
                                    float* ctx_last, float* prob, int B, int L, int d, int H, b2r_stream_t stream);
 B2R_API int b2r_attention_last_bwd(const float* q_last, const float* k, const float* v, int ld, const int64_t* lengths,
@@ -364,11 +350,10 @@ B2R_API int b2r_small_table_grad(const float* src, int ld, const int64_t* ids, i
 
 /* Training envelope of SASRec: 0 when every kernel of a training step (forward and backward) accepts batches of width
  * 1..L at embedding width d with H heads, else B2R_E_UNSUPPORTED with b2r_last_error() naming the refusing kernel and its
- * limit.  full_blocks = the blocks that run full causal attention; flags: B2R_SEQ_LAST_QUERY when the last block runs for
- * the one query per sequence (b2r_attention_last_*), B2R_SEQ_ATTN_V1 when full attention always takes the shared-memory
- * kernels (b2r_attention_*_live) instead of trying b2r_attention_*_rt first.  Host only: no device call is made. */
+ * limit.  full_blocks = the blocks that run full causal attention (b2r_attention_*_rt where it applies, else
+ * b2r_attention_*_live); flags: B2R_SEQ_LAST_QUERY when the last block runs for the one query per sequence
+ * (b2r_attention_last_*); any other flag bit is B2R_E_BADARG.  Host only: no device call is made. */
 #define B2R_SEQ_LAST_QUERY 1
-#define B2R_SEQ_ATTN_V1 2
 B2R_API int b2r_seq_train_check(int L, int d, int H, int full_blocks, int flags);
 
 /* out[r,k] = a[r,k] * w[k]   and   out[k] = sum_r a[r,k] * b[r,k]   (the GMF half of NeuMF's final Linear,

@@ -372,12 +372,12 @@ extern "C" int b2r_embed_history(const float* I, int64_t n_items, const float* P
 
 extern "C" int b2r_attention_fwd_live(const float* q, const float* k, const float* v, int ld, const int64_t* live, float* ctx,
                                       int B, int L, int d, int H, b2r_stream_t stream) {
-    B2R_REQUIRE(q && k && v && ctx, B2R_E_BADARG, "b2r_attention_fwd: null pointer");
+    B2R_REQUIRE(q && k && v && ctx, B2R_E_BADARG, "b2r_attention_fwd_live: null pointer");
     B2R_REQUIRE(B >= 0 && L > 0 && d > 0 && H > 0 && d % H == 0 && ld >= d, B2R_E_BADARG,
-                "b2r_attention_fwd: bad shape B=%d L=%d d=%d H=%d ld=%d", B, L, d, H, ld);
+                "b2r_attention_fwd_live: bad shape B=%d L=%d d=%d H=%d ld=%d", B, L, d, H, ld);
     if (B == 0) return 0;
     const size_t smem = attn_fwd_smem(L, d, H);
-    B2R_REQUIRE(smem <= kAttnSmemMax, B2R_E_UNSUPPORTED, "b2r_attention_fwd: L=%d d=%d needs %zu B of shared memory", L, d,
+    B2R_REQUIRE(smem <= kAttnSmemMax, B2R_E_UNSUPPORTED, "b2r_attention_fwd_live: L=%d d=%d needs %zu B of shared memory", L, d,
                 smem);
     B2R_CUDA_OK(cudaFuncSetAttribute(k_attention_fwd, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     k_attention_fwd<<<B, 256, smem, as_stream(stream)>>>(q, k, v, ld, ctx, L, d, H, 1.f / sqrtf((float)(d / H)), live);
@@ -385,31 +385,21 @@ extern "C" int b2r_attention_fwd_live(const float* q, const float* k, const floa
     return 0;
 }
 
-extern "C" int b2r_attention_fwd(const float* q, const float* k, const float* v, int ld, float* ctx, int B, int L,
-                                 int d, int H, b2r_stream_t stream) {
-    return b2r_attention_fwd_live(q, k, v, ld, nullptr, ctx, B, L, d, H, stream);
-}
-
 extern "C" int b2r_attention_bwd_live(const float* q, const float* k, const float* v, int ld, const int64_t* live,
                                       const float* dctx, float* dq, float* dk, float* dv, int ldg, int B, int L, int d, int H,
                                       b2r_stream_t stream) {
-    B2R_REQUIRE(q && k && v && dctx && dq && dk && dv, B2R_E_BADARG, "b2r_attention_bwd: null pointer");
+    B2R_REQUIRE(q && k && v && dctx && dq && dk && dv, B2R_E_BADARG, "b2r_attention_bwd_live: null pointer");
     B2R_REQUIRE(B >= 0 && L > 0 && L <= kAttnBwdMaxL && d > 0 && H > 0 && d % H == 0 && ld >= d && ldg >= d, B2R_E_BADARG,
-                "b2r_attention_bwd: bad shape B=%d L=%d d=%d H=%d", B, L, d, H);
+                "b2r_attention_bwd_live: bad shape B=%d L=%d d=%d H=%d", B, L, d, H);
     if (B == 0) return 0;
     const size_t smem = attn_bwd_smem(L, d, H);
-    B2R_REQUIRE(smem <= kAttnSmemMax, B2R_E_UNSUPPORTED, "b2r_attention_bwd: L=%d d=%d H=%d needs %zu B of shared memory",
+    B2R_REQUIRE(smem <= kAttnSmemMax, B2R_E_UNSUPPORTED, "b2r_attention_bwd_live: L=%d d=%d H=%d needs %zu B of shared memory",
                 L, d, H, smem);
     B2R_CUDA_OK(cudaFuncSetAttribute(k_attention_bwd, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     k_attention_bwd<<<B, 256, smem, as_stream(stream)>>>(q, k, v, ld, dctx, dq, dk, dv, ldg, L, d, H,
                                                         1.f / sqrtf((float)(d / H)), live);
     B2R_LAUNCH_OK("k_attention_bwd");
     return 0;
-}
-
-extern "C" int b2r_attention_bwd(const float* q, const float* k, const float* v, int ld, const float* dctx, float* dq,
-                                 float* dk, float* dv, int ldg, int B, int L, int d, int H, b2r_stream_t stream) {
-    return b2r_attention_bwd_live(q, k, v, ld, nullptr, dctx, dq, dk, dv, ldg, B, L, d, H, stream);
 }
 
 extern "C" int b2r_select_last(const float* y, const int64_t* hist, const int64_t* lengths, float* h, int B, int L,

@@ -1,5 +1,4 @@
-// attention_last.cu -- SASRec's last block for one query per sequence (the default route; B2R_SASREC_LASTQ=0 runs the
-// full block instead).  Batch widths up to kALMaxL = 256 (seq_limits.cuh).
+// attention_last.cu -- SASRec's last block for one query per sequence.  Batch widths up to kALMaxL = 256 (seq_limits.cuh).
 //
 // SASRec scores candidates against ONE vector per sequence: the encoder state at position len-1 of the LAST block
 // (models/sequential/SASRec.py:74-81).  Every other position of the last block's output is dead, so for that block

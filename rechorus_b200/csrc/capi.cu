@@ -1,4 +1,4 @@
-// capi.cu -- version / error / device-info entry points of libb200rec.so
+// capi.cu -- version / error / measurement entry points of libb200rec.so
 #include "common.cuh"
 
 namespace b2r {
@@ -61,22 +61,3 @@ extern "C" int b2r_profile_arm(int tag, void* ev_start, void* ev_stop) {
 extern "C" int b2r_version(void) { return B2R_VERSION; }
 
 extern "C" const char* b2r_last_error(void) { return b2r::err_buf(); }
-
-extern "C" int b2r_device_info(int* sm_count, int* cc_major, int* cc_minor) {
-    int dev = 0;
-    B2R_CUDA_OK(cudaGetDevice(&dev));
-    int v = 0;
-    if (sm_count) {
-        B2R_CUDA_OK(cudaDeviceGetAttribute(&v, cudaDevAttrMultiProcessorCount, dev));
-        *sm_count = v;
-    }
-    if (cc_major) {
-        B2R_CUDA_OK(cudaDeviceGetAttribute(&v, cudaDevAttrComputeCapabilityMajor, dev));
-        *cc_major = v;
-    }
-    if (cc_minor) {
-        B2R_CUDA_OK(cudaDeviceGetAttribute(&v, cudaDevAttrComputeCapabilityMinor, dev));
-        *cc_minor = v;
-    }
-    return 0;
-}

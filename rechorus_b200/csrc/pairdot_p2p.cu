@@ -1,5 +1,5 @@
-// pairdot_p2p.cu -- groundwork for the fused compute+exchange form of config 5 (DESIGN.md §8; opt-in via
-// B2R_SHARD_P2P=1, not yet run on a GPU).  Same scoring as k_pairdot_fwd (pairdot.cu): out = <Q[qidx[e]], T[rows[e]]>
+// pairdot_p2p.cu -- the scoring hop of config 5's fused compute+exchange form (DESIGN.md §8; the default exchange,
+// ShardedBPRMF exchange="p2p").  Same scoring as k_pairdot_fwd (pairdot.cu): out = <Q[qidx[e]], T[rows[e]]>
 // for the (sample, local row) pairs an item-shard owner received -- but the score of pair e, which belongs to source
 // rank s = e / seg, is stored straight into THAT rank's receive buffer through its peer-mapped pointer
 // (out_tab[s] + e % seg; NVLink stores), so the scores need no all-to-all of their own: a signal-pad barrier after the

@@ -71,29 +71,22 @@ extern "C" size_t b2r_plan_workspace_bytes(int64_t n, int64_t n_rows) {
     return L.total;
 }
 
-extern "C" int b2r_plan_build(const int64_t* ids, int64_t n, int64_t n_rows, uint32_t* sorted_key,
-                              uint32_t* sorted_pos, int32_t* seg_start, int32_t* n_uniq, void* ws,
-                              size_t ws_bytes, int32_t* err_flag, b2r_stream_t stream) {
-    return b2r_plan_build_ex(ids, n, n_rows, -1, 0, sorted_key, sorted_pos, seg_start, n_uniq, ws, ws_bytes, err_flag,
-                             stream);
-}
-
 extern "C" int b2r_plan_build_ex(const int64_t* ids, int64_t n, int64_t n_rows, int64_t ignore_id, int64_t ignore_n,
                                  uint32_t* sorted_key, uint32_t* sorted_pos, int32_t* seg_start, int32_t* n_uniq,
                                  void* ws, size_t ws_bytes, int32_t* err_flag, b2r_stream_t stream) {
     B2R_REQUIRE(ids && sorted_key && sorted_pos && seg_start && n_uniq && ws, B2R_E_BADARG,
-                "b2r_plan_build: null pointer");
-    B2R_REQUIRE(n > 0 && n <= 0x7fffffff, B2R_E_BADARG, "b2r_plan_build: n must be in [1, 2^31) (n=%lld)",
+                "b2r_plan_build_ex: null pointer");
+    B2R_REQUIRE(n > 0 && n <= 0x7fffffff, B2R_E_BADARG, "b2r_plan_build_ex: n must be in [1, 2^31) (n=%lld)",
                 (long long)n);
     B2R_REQUIRE(n_rows > 0 && n_rows < 0xffffffffLL, B2R_E_UNSUPPORTED,
-                "b2r_plan_build: n_rows must fit 32 bits (n_rows=%lld)", (long long)n_rows);
+                "b2r_plan_build_ex: n_rows must fit 32 bits (n_rows=%lld)", (long long)n_rows);
     PlanLayout L;
     int rc = plan_layout(n, n_rows, &L);
     if (rc != 0) return rc;
-    B2R_REQUIRE(ws_bytes >= L.total, B2R_E_WORKSPACE, "b2r_plan_build: workspace %zu < required %zu", ws_bytes,
+    B2R_REQUIRE(ws_bytes >= L.total, B2R_E_WORKSPACE, "b2r_plan_build_ex: workspace %zu < required %zu", ws_bytes,
                 L.total);
     B2R_REQUIRE((reinterpret_cast<uintptr_t>(ws) & 255u) == 0, B2R_E_BADARG,
-                "b2r_plan_build: workspace must be 256-byte aligned");
+                "b2r_plan_build_ex: workspace must be 256-byte aligned");
     cudaStream_t s = as_stream(stream);
     char* base = static_cast<char*>(ws);
     uint32_t* key_in = reinterpret_cast<uint32_t*>(base + L.key_in);

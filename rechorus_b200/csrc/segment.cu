@@ -1,5 +1,5 @@
 // segment.cu -- row-sparse embedding backward over an index plan, optionally fused with the optimizer step
-// (the other half of K2), plus the atomic scatter alternative and the dense optimizer.
+// (the other half of K2), plus the dense optimizer.
 //
 // One lane group (LPR = d/4 lanes, one float4 each) owns one unique table row.  It walks the row's
 // contributions in ascending batch position, accumulates in registers, and then either writes the
@@ -232,27 +232,6 @@ k_segment_apply_generic(const uint32_t* __restrict__ sorted_key, const uint32_t*
     }
 }
 
-// dense[ids[p / 1]] += coef[p] * src[row(p)] with vector reductions (order-nondeterministic)
-__global__ void __launch_bounds__(256)
-k_scatter_add_atomic(const int64_t* __restrict__ ids, int64_t n_rows, Src s, int d, float* __restrict__ dense,
-                     int32_t* err_flag) {
-    const int lane = threadIdx.x & 31;
-    const int d4 = d >> 2;
-    for (int64_t p = (int64_t)blockIdx.x * 8 + (threadIdx.x >> 5); p < s.n; p += (int64_t)gridDim.x * 8) {
-        const int64_t dst = checked_id(ids[p], n_rows, lane == 0 ? err_flag : nullptr);
-        int64_t r = (s.div == 1) ? p : p / s.div;
-        if (s.src_id != nullptr) r = s.src_id[r];
-        const float c = (s.coef != nullptr) ? s.coef[p] : 1.f;
-        for (int k = lane; k < d4; k += 32) {
-            const float4 x = ld4(s.src + r * s.ld + k * 4);
-            float* a = dense + dst * d + k * 4;
-            asm volatile("red.global.add.v4.f32 [%0], {%1, %2, %3, %4};" ::"l"(a), "f"(c * x.x), "f"(c * x.y),
-                         "f"(c * x.z), "f"(c * x.w)
-                         : "memory");
-        }
-    }
-}
-
 __global__ void __launch_bounds__(256)
 k_dense_optim(float* __restrict__ W, const float* __restrict__ G, float* __restrict__ M, float* __restrict__ V,
               int64_t numel, OptK opt) {
@@ -372,20 +351,6 @@ extern "C" int b2r_segment_apply(const uint32_t* sorted_key, const uint32_t* sor
 #undef B2R_SEG_D
 #undef B2R_SEG
     B2R_LAUNCH_OK("k_segment_apply");
-    return 0;
-}
-
-extern "C" int b2r_scatter_add_atomic(const int64_t* ids, int64_t n_rows, const b2r_grad_source* src, int d,
-                                      float* dense, int32_t* err_flag, b2r_stream_t stream) {
-    B2R_REQUIRE(ids && src && src->src && dense, B2R_E_BADARG, "b2r_scatter_add_atomic: null pointer");
-    B2R_REQUIRE(d > 0 && d % 4 == 0 && n_rows > 0, B2R_E_BADARG, "b2r_scatter_add_atomic: bad d or n_rows");
-    if (src->n <= 0) return 0;
-    const Src a = to_src(src, d);
-    int64_t need = (a.n + 7) / 8;
-    const int64_t cap = (int64_t)sm_count() * 16;
-    k_scatter_add_atomic<<<(int)(need < cap ? need : cap), 256, 0, as_stream(stream)>>>(ids, n_rows, a, d, dense,
-                                                                                       err_flag);
-    B2R_LAUNCH_OK("k_scatter_add_atomic");
     return 0;
 }
 

@@ -42,14 +42,13 @@ class Dropout(C.Structure):
 
 
 OPT_SGD, OPT_ADAM, OPT_ADAGRAD = 0, 1, 2
-SEQ_LAST_QUERY, SEQ_ATTN_V1 = 1, 2          # b2r_seq_train_check flags
+SEQ_LAST_QUERY = 1                          # b2r_seq_train_check flag
 PROF_SCORE_FWD, PROF_SCORE_BWDQ, PROF_SEGMENT_I, PROF_SEGMENT_U, PROF_PLAN_I, PROF_LOSS = range(6)
 
 # name -> (restype, argtypes); must list every symbol include/b200rec.h declares (tests/test_abi.py checks)
 SIGNATURES = {
     "b2r_version": (C.c_int, []),
     "b2r_last_error": (C.c_char_p, []),
-    "b2r_device_info": (C.c_int, [C.POINTER(C.c_int)] * 3),
     "b2r_launch_count": (C.c_longlong, []),
     "b2r_profile_arm": (C.c_int, [C.c_int, C.c_void_p, C.c_void_p]),
     "b2r_rowdot_fwd": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p, C.c_int64,
@@ -64,8 +63,6 @@ SIGNATURES = {
                                     C.c_int64, C.c_int, C.c_void_p]),
     "b2r_bpr_loss": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_void_p]),
     "b2r_plan_workspace_bytes": (C.c_size_t, [C.c_int64, C.c_int64]),
-    "b2r_plan_build": (C.c_int, [C.c_void_p, C.c_int64, C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p,
-                                 C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p, C.c_void_p]),
     "b2r_plan_build_ex": (C.c_int, [C.c_void_p, C.c_int64, C.c_int64, C.c_int64, C.c_int64, C.c_void_p, C.c_void_p,
                                     C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p, C.c_void_p]),
     "b2r_gather_rows_strided": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p, C.c_int, C.c_int64,
@@ -81,8 +78,6 @@ SIGNATURES = {
     "b2r_direct_plan_apply": (C.c_int, [C.c_void_p, C.c_int64, C.c_int64, C.c_int, C.POINTER(GradSource),
                                         C.POINTER(GradSource), C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
                                         C.POINTER(Optim), C.c_void_p]),
-    "b2r_scatter_add_atomic": (C.c_int, [C.c_void_p, C.c_int64, C.POINTER(GradSource), C.c_int, C.c_void_p,
-                                         C.c_void_p, C.c_void_p]),
     "b2r_optim_tick": (C.c_int, [C.c_void_p, C.c_float, C.c_double, C.c_double, C.c_void_p]),
     "b2r_dense_optim": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64,
                                   C.POINTER(Optim), C.c_void_p]),
@@ -122,11 +117,6 @@ SIGNATURES = {
                                                                     C.c_size_t, C.c_void_p]),
     "b2r_embed_history": (C.c_int, [C.c_void_p, C.c_int64, C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p,
                                     C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p]),
-    "b2r_attention_fwd": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.c_int,
-                                    C.c_int, C.c_int, C.c_void_p]),
-    "b2r_attention_bwd": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p,
-                                    C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int,
-                                    C.c_void_p]),
     "b2r_attention_fwd_live": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_int, C.c_int,
                                          C.c_int, C.c_int, C.c_void_p]),
     "b2r_attention_bwd_live": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p,

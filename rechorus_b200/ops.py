@@ -13,8 +13,6 @@ Embedding-table gradients can leave the autograd graph in three forms, selected 
 """
 from __future__ import annotations
 
-import os
-
 import ctypes as C
 from dataclasses import dataclass
 from typing import List, Optional, Sequence, Tuple
@@ -151,7 +149,7 @@ def pairdot(Q: torch.Tensor, qidx: torch.Tensor, T: torch.Tensor, rows: torch.Te
 def pairdot_p2p(Q: torch.Tensor, qidx: torch.Tensor, T: torch.Tensor, rows: torch.Tensor, out_tab: torch.Tensor,
                 seg: int) -> None:
     """pairdot whose score for pair e goes to out_tab[e // seg][e % seg]; out_tab: int64 device tensor of float*
-    addresses (peer-mapped receive buffers).  Opt-in groundwork for the fused exchange of config 5 (b2r_pairdot_fwd_p2p)."""
+    addresses (peer-mapped receive buffers).  The scoring hop of config 5's default exchange (b2r_pairdot_fwd_p2p)."""
     _need_cuda(Q, qidx, T, rows, out_tab)
     Q, T = _f32c(Q, "Q"), _f32c(T, "T")
     qidx, rows = _i64c(qidx.reshape(-1), "qidx"), _i64c(rows.reshape(-1), "rows")
@@ -536,7 +534,7 @@ class Source:
 
 
 class IndexPlan:
-    """Sorted, de-duplicated view of the ids a batch touches in one table (b2r_plan_build)."""
+    """Sorted, de-duplicated view of the ids a batch touches in one table (b2r_plan_build_ex)."""
 
     def __init__(self, ids: torch.Tensor, n_rows: int, ignore_id: int = -1, ignore_n: int = 0):
         _need_cuda(ids)
@@ -655,15 +653,6 @@ def make_plan(ids: torch.Tensor, n_rows: int, d: int, ignore_id: int = -1, ignor
     if d in DirectPlan.SUPPORTED_D and DirectPlan.available(ids.numel(), n_rows):
         return DirectPlan(ids, n_rows, ignore_id, ignore_n)
     return IndexPlan(ids, n_rows, ignore_id, ignore_n)
-
-
-def scatter_add_atomic(dense: torch.Tensor, ids: torch.Tensor, source: Source) -> None:
-    """order-nondeterministic dense += via red.global.add.v4.f32 (b2r_scatter_add_atomic)"""
-    ids = _i64c(ids.reshape(-1), "ids")
-    s = source.c_struct()
-    L = _lib.load()
-    _lib.check(L.b2r_scatter_add_atomic(_p(ids), dense.shape[0], C.byref(s), dense.shape[1], _p(dense),
-                                        _p(err_flag(dense.device)), _stream()), "b2r_scatter_add_atomic")
 
 
 def dense_optim(W: torch.Tensor, grad: torch.Tensor, m, v, opt: _lib.Optim) -> None:
@@ -1061,7 +1050,7 @@ def linear_bwd(dy: torch.Tensor, x: torch.Tensor, W: torch.Tensor, y_relu: Optio
         dx = torch.empty((M, K), dtype=torch.float32, device=dy.device)
         done = False
         Wd = W if drop is None else W * drop.scale
-        if _TC_LINEAR and M >= 4096 and N % 32 == 0 and N <= 128 and K % 16 == 0 and K <= 256 and lddy % 4 == 0:
+        if M >= 4096 and N % 32 == 0 and N <= 128 and K % 16 == 0 and K <= 256 and lddy % 4 == 0:
             # dX = (dY o mask) W = (dY o mask) (W^T)^T on the tensor-core kernel: the transposed weight (N*K floats) is a copy
             Wt = Wd.t().contiguous()
             rc = L.b2r_linear_tc(_p(dy), lddy, _p(y_relu), _p(Wt), None, _p(dx), K, M, K, N, 0, _stream())
@@ -1074,7 +1063,7 @@ def linear_bwd(dy: torch.Tensor, x: torch.Tensor, W: torch.Tensor, y_relu: Optio
     if need_dw or need_db:
         dW = torch.empty((N, K), dtype=torch.float32, device=dy.device)
         db = torch.empty((N,), dtype=torch.float32, device=dy.device) if need_db else None
-        if _TC_DW and M >= 4096 and N % 4 == 0 and N <= 128 and K % 16 == 0 and K <= 240 and lddy % 4 == 0 and ldx % 4 == 0:
+        if M >= 4096 and N % 4 == 0 and N <= 128 and K % 16 == 0 and K <= 240 and lddy % 4 == 0 and ldx % 4 == 0:
             # long reductions (M = B*L rows) on the tensor cores: k_linear_dw_tc
             ws = _ws(L.b2r_linear_bwd_weight_tc_workspace_bytes(M, N, K), dy.device)
             if drop is None:
@@ -1101,13 +1090,6 @@ def linear_bwd(dy: torch.Tensor, x: torch.Tensor, W: torch.Tensor, y_relu: Optio
     return dx, dW, db
 
 
-# Linear forward and dX with a long batch dimension (M >= 4096) run on the tensor cores (csrc/linear_tc.cu: wgmma, TF32
-# hi/lo split, 3 products, fp32-class accuracy checked in tests/test_gpu_tc.py); B2R_TC_LINEAR=0: CUDA-core SGEMM everywhere
-_TC_LINEAR = os.environ.get("B2R_TC_LINEAR", "1") != "0"
-# weight gradients with a long batch reduction run on the tensor cores (csrc/linear_dw_tc.cu); B2R_TC_DW=0: CUDA cores
-_TC_DW = os.environ.get("B2R_TC_DW", "1") != "0"
-
-
 class _Linear(torch.autograd.Function):
     """nn.Linear (+ optional ReLU, + optional dropout after the ReLU) on the library's SGEMM: NeuMF.py:70-71 /
     layers.py:26-28,106-107."""
@@ -1119,7 +1101,9 @@ class _Linear(torch.autograd.Function):
         if x2.stride(1) != 1:
             x2 = x2.contiguous()
         N, K = W.shape
-        tc = _TC_LINEAR and x2.shape[0] >= 4096 and K % 32 == 0 and K <= 128 and N % 16 == 0 and N <= 256
+        # a long batch dimension (M >= 4096) runs on the tensor cores (csrc/linear_tc.cu: wgmma, TF32 hi/lo split,
+        # 3 products, fp32-class accuracy checked in tests/test_gpu_tc.py); linear_bwd picks dX and dW the same way
+        tc = x2.shape[0] >= 4096 and K % 32 == 0 and K <= 128 and N % 16 == 0 and N <= 256
         if drop is not None:
             if not relu:
                 raise ValueError("fused dropout follows a ReLU (its backward reads the mask off the saved output)")
@@ -1213,10 +1197,6 @@ def add_layernorm(x, res, gamma, beta, eps=1e-5, drop: Optional[Drop] = None, le
     return _AddLayerNorm.apply(x, res, gamma, beta, eps, drop, lengths, int(seq_len))
 
 
-# B2R_ATTN=v1: the first (shared-memory operand) attention kernels for every shape, for A/B
-_ATTN_RT = os.environ.get("B2R_ATTN", "rt") != "v1"
-
-
 class _CausalAttention(torch.autograd.Function):
     """layers.py:52-63 for q,k,v [B, L, d] with H heads (contiguous d/H chunks), causal mask, no W_o.  ``live`` (optional
     int64 [B]): positions >= live[b] are dead rows (nothing downstream reads them): skipped, written as zeros."""
@@ -1230,7 +1210,7 @@ class _CausalAttention(torch.autograd.Function):
         out = torch.empty((B, Ln, d), dtype=torch.float32, device=q.device)
         L = _lib.load()
         lse = None
-        if _ATTN_RT and d % H == 0 and d // H in (8, 16, 32) and Ln <= 128:
+        if d % H == 0 and d // H in (8, 16, 32) and Ln <= 128:
             # register-resident kernels (csrc/attention_rt.cu); the row log-sum-exp is kept for the backward
             lse = torch.empty((B, Ln, H), dtype=torch.float32, device=q.device)
             rc = L.b2r_attention_fwd_rt(_p(q), _p(k), _p(v), d, _p(live), _p(out), _p(lse), B, Ln, d, H, _stream())
@@ -1238,9 +1218,9 @@ class _CausalAttention(torch.autograd.Function):
                 lse = None
             else:
                 _lib.check(rc, "b2r_attention_fwd_rt")
-        if lse is None:
+        if lse is None:                                    # shared-memory kernels (csrc/attention.cu)
             _lib.check(L.b2r_attention_fwd_live(_p(q), _p(k), _p(v), d, _p(live), _p(out), B, Ln, d, H, _stream()),
-                       "b2r_attention_fwd")
+                       "b2r_attention_fwd_live")
         ctx.save_for_backward(q, k, v, live, out if lse is not None else None, lse)
         ctx.H = H
         return out
@@ -1257,7 +1237,7 @@ class _CausalAttention(torch.autograd.Function):
                                               _p(dv), d, B, Ln, d, ctx.H, _stream()), "b2r_attention_bwd_rt")
         else:
             _lib.check(L.b2r_attention_bwd_live(_p(q), _p(k), _p(v), d, _p(live), _p(dout), _p(dq), _p(dk), _p(dv), d, B, Ln,
-                                                d, ctx.H, _stream()), "b2r_attention_bwd")
+                                                d, ctx.H, _stream()), "b2r_attention_bwd_live")
         return dq, dk, dv, None, None
 
 
@@ -1266,11 +1246,10 @@ def causal_attention(q, k, v, num_heads, live=None):
 
 
 def seq_train_error(L: int, d: int, H: int, num_layers: int, last_query: bool) -> Optional[str]:
-    """None when a SASRec training step on batches of width up to L runs on the kernels (b2r_seq_train_check, with the
-    attention route this process takes), else the library's reason.  last_query: the last block runs for the one query
-    per sequence (attention_last)."""
+    """None when a SASRec training step on batches of width up to L runs on the kernels (b2r_seq_train_check), else the
+    library's reason.  last_query: the last block runs for the one query per sequence (attention_last)."""
     last_query = bool(last_query) and num_layers > 0
-    flags = (_lib.SEQ_LAST_QUERY if last_query else 0) | (0 if _ATTN_RT else _lib.SEQ_ATTN_V1)
+    flags = _lib.SEQ_LAST_QUERY if last_query else 0
     L_ = _lib.load()
     rc = L_.b2r_seq_train_check(int(L), int(d), int(H), int(num_layers) - int(last_query), flags)
     return None if rc == 0 else L_.b2r_last_error().decode("utf-8", "replace")
@@ -1278,8 +1257,7 @@ def seq_train_error(L: int, d: int, H: int, num_layers: int, last_query: bool) -
 
 class _AttentionLast(torch.autograd.Function):
     """Attention for the one query per sequence that SASRec's last block needs (position len-1): q_last [B, d] against
-    k, v [B, L, d]; identical to row len-1 of _CausalAttention.  SASRec's last block runs on it by default
-    (B2R_SASREC_LASTQ=0 runs the full block instead); L <= 256."""
+    k, v [B, L, d]; identical to row len-1 of _CausalAttention.  SASRec's last block runs on it; L <= 256."""
 
     @staticmethod
     def forward(ctx, q_last, k, v, lengths, H):

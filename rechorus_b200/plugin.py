@@ -32,12 +32,9 @@ from . import ops
 # ======================================================================================================
 
 
-# SASRec's last block is computed for the one query per sequence whose output is used (exact; 7.56 -> 5.32 ms per
-# config-4 step, profiles/README r2).  B2R_SASREC_LASTQ=0 runs the full block instead (A/B).
-_SASREC_LASTQ = os.environ.get("B2R_SASREC_LASTQ", "1") != "0"
-# Attention rows at positions >= len are dead work (the model reads position len-1 only, SASRec.py:74-81, and the mask is
-# causal): skipped exactly.  B2R_SASREC_LIVE=0 computes them as the reference does (A/B).
-_SASREC_LIVE = os.environ.get("B2R_SASREC_LIVE", "1") != "0"
+# SASRec's last block runs for the one query per sequence whose output is used (exact); tests set this False for the
+# full last block, the reference they compare against.
+_SASREC_LASTQ = True
 
 
 class _KernelModelMixin:
@@ -426,7 +423,9 @@ class SASRecKernels(_KernelModelMixin):
             q = ops.linear(x, a.q_linear.weight, a.q_linear.bias)
             k = ops.linear(x, a.k_linear.weight, a.k_linear.bias)
             v = ops.linear(x, a.v_linear.weight, a.v_linear.bias)
-            ctx = ops.causal_attention(q, k, v, self.num_heads, live=lengths if _SASREC_LIVE else None)
+            # rows at positions >= len are dead work (the model reads position len-1 only, SASRec.py:74-81, and the
+            # mask is causal): skipped exactly
+            ctx = ops.causal_attention(q, k, v, self.num_heads, live=lengths)
             c = ops.add_layernorm(ctx, x, blk.layer_norm1.weight, blk.layer_norm1.bias, drop=d1)       # dropout1 fused
             o = ops.linear(ops.linear(c, blk.linear1.weight, blk.linear1.bias, relu=True),
                            blk.linear2.weight, blk.linear2.bias)

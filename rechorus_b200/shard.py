@@ -39,7 +39,6 @@ Two forms of the exchange:
 from __future__ import annotations
 
 import math
-import os
 from typing import Optional
 
 import torch
@@ -105,9 +104,12 @@ def _bucket_by_owner(owner: torch.Tensor, world: int):
 class ShardedBPRMF:
     def __init__(self, n_users: int, n_items: int, d: int, device, backend=None, group=None, optimizer: str = "Adam",
                  lr: float = 1e-3, l2: float = 0.0, betas=(0.9, 0.999), eps: Optional[float] = None,
-                 cap_factor: float = 1.25, seed: int = 0, init_std: float = 0.01, world_override: Optional[int] = None):
+                 cap_factor: float = 1.25, seed: int = 0, init_std: float = 0.01, world_override: Optional[int] = None,
+                 exchange: Optional[str] = None):
         """world_override=1: hold the WHOLE table on this rank and exchange nothing even inside an initialised process
-        group (the 1-GPU anchor of the scaling curve, run by one rank while the others wait)"""
+        group (the 1-GPU anchor of the scaling curve, run by one rank while the others wait).
+        exchange: "p2p" or "nccl" (module docstring); None picks "p2p" on CUDA without an injected backend, else
+        "nccl".  "p2p" runs the library kernels on CUDA memory, so it needs both."""
         self.group = group
         self.world = dist.get_world_size(group) if dist.is_initialized() else 1
         self.rank = dist.get_rank(group) if dist.is_initialized() else 0
@@ -123,9 +125,14 @@ class ShardedBPRMF:
         self.eps = {"SGD": 0.0, "Adam": 1e-8, "Adagrad": 1e-10}[optimizer] if eps is None else eps
         self.cap_factor = cap_factor
         self.t = 0
-        want = os.environ.get("B2R_SHARD_EXCHANGE", "p2p")
-        is_cuda = torch.device(device).type == "cuda"
-        self.exchange = "p2p" if (is_cuda and backend is None and want != "nccl") else "nccl"
+        p2p_ok = torch.device(device).type == "cuda" and backend is None
+        if exchange is None:
+            exchange = "p2p" if p2p_ok else "nccl"
+        elif exchange not in ("p2p", "nccl"):
+            raise ValueError(f"exchange must be 'p2p' or 'nccl', got {exchange!r}")
+        elif exchange == "p2p" and not p2p_ok:
+            raise ValueError("exchange='p2p' needs a CUDA device and the library backend")
+        self.exchange = exchange
         self._p2p = None
         g = torch.Generator(device=device).manual_seed(seed * 1000 + self.rank)
         # models/BaseModel.py:29-35 init, one shard per rank
@@ -137,31 +144,6 @@ class ShardedBPRMF:
                 st["m"] = torch.zeros_like(W)
             if optimizer != "SGD":
                 st["v"] = torch.zeros_like(W)
-
-    # -- opt-in groundwork (B2R_SHARD_P2P=1, not yet run on a GPU): scores returned by peer stores ----------
-    def _peer_scores(self, cap: int):
-        """Symmetric [W, cap] float32 score buffer + the device table of peer pointers this rank writes through
-        (entry s = rank s's buffer, row `my rank`).  Returns None when the feature is off or cannot be set up -- the
-        caller then uses the NCCL all-to-all."""
-        if not (os.environ.get("B2R_SHARD_P2P") == "1" and self.world > 1 and self.U.is_cuda):
-            return None
-        cache = self.__dict__.setdefault("_p2p_cache", {})
-        if cap in cache:
-            return cache[cap]
-        try:
-            import torch.distributed._symmetric_memory as symm
-            W = self.world
-            buf = symm.empty(W * cap, dtype=torch.float32, device=self.U.device)
-            hdl = symm.rendezvous(buf, self.group if self.group is not None else dist.group.WORLD)
-            me = dist.get_rank(self.group)
-            ptrs = [int(hdl.buffer_ptrs[s]) + me * cap * 4 for s in range(W)]
-            tab = torch.tensor(ptrs, dtype=torch.int64, device=self.U.device)
-            cache[cap] = (hdl, buf.view(W, cap), tab)
-        except Exception as e:                                # pragma: no cover - depends on the box
-            import warnings
-            warnings.warn(f"B2R_SHARD_P2P: symmetric memory unavailable ({e!r}); using the NCCL exchange")
-            cache[cap] = None
-        return cache[cap]
 
     # -- collectives (degenerate to copies for a single rank) --------------------------------------------
     def _a2a(self, x: torch.Tensor) -> torch.Tensor:
@@ -247,18 +229,7 @@ class ShardedBPRMF:
         qidx = (recv_pairs & ((1 << 21) - 1)) + src_base                          # row of q_all (garbage where rows < 0)
         qidx = torch.where(rows >= 0, qidx, torch.zeros_like(qidx))
         # D. owners score, scores travel back
-        p2p = self._peer_scores(cap)
-        if p2p is None:
-            sc_recv = self._a2a(be.pairdot(q_all, qidx, self.I, rows).view(W, cap))   # [W(owner), cap]
-        else:
-            # fused compute + exchange: the owner's scoring kernel stores each score into the requester's buffer over
-            # NVLink; the barriers order those stores against the requester's reads (before: nobody still reads the
-            # previous step's scores; after: every owner's stores have landed)
-            hdl, local, tab = p2p
-            hdl.barrier(channel=0)
-            be.pairdot_p2p(q_all, qidx, self.I, rows, tab, cap)
-            hdl.barrier(channel=1)
-            sc_recv = local                                                          # [W(owner), cap]
+        sc_recv = self._a2a(be.pairdot(q_all, qidx, self.I, rows).view(W, cap))   # [W(owner), cap]
         pred = torch.empty(n, dtype=torch.float32, device=dev)
         pred[ord_i] = sc_recv[own_is, keep_rank]
         state = dict(B=B, C=C, n=n, cap=cap, ord_u=ord_u, own_us=own_us, rank_u=rank_u, recv_uid=recv_uid,

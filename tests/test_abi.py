@@ -30,11 +30,11 @@ def test_library_exports_every_declared_symbol(built_lib):
         assert hasattr(lib, name), f"{name} declared in include/b200rec.h but not exported"
 
 
-def test_binding_table_matches_header_at_abi_version_102(built_lib):
+def test_binding_table_matches_header_at_abi_version_103(built_lib):
     from rechorus_b200 import lib as L
     assert sorted(L.SIGNATURES) == _declared()
     handle = L.load()
-    assert handle.b2r_version() == 102
+    assert handle.b2r_version() == 103
     assert ctypes.sizeof(L.GradSource) == 40 and ctypes.sizeof(L.Optim) == 48      # b2r_optim: 9 x 4 bytes, pad, clock pointer
 
 

@@ -225,20 +225,6 @@ def test_fused_row_sparse_optimizer_equals_lazy_reference_update(name):
             assert (p.detach().cpu() - cpu_w[k]).abs().max() <= 2e-6, (name, t, k)
 
 
-def test_atomic_scatter_matches_deterministic_scatter():
-    from rechorus_b200 import ops
-    g = torch.Generator().manual_seed(8)
-    ids = torch.randint(0, 50, (16, 12), generator=g).cuda()
-    q = torch.randn(16, 64, generator=g).cuda()
-    coef = torch.randn(16 * 12, generator=g).cuda()
-    src = ops.Source(src=q, n=16 * 12, coef=coef, div=12)
-    a = torch.zeros(50, 64).cuda()
-    ops.scatter_add_atomic(a, ids, src)
-    b = torch.zeros(50, 64).cuda()
-    ops.IndexPlan(ids, 50).add_to_dense(b, [src])
-    assert (a - b).abs().max() <= 1e-5
-
-
 def test_full_size_config2_properties():
     """BASELINE config 2 shapes (1 M items, d=64, B=4096, K=99): size-independent properties + a torch fp32
     check on the same device."""

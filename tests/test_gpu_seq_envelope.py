@@ -70,14 +70,12 @@ RT_CASES = [(3, 1, 32, 4), (3, 31, 64, 4), (3, 32, 96, 3), (3, 33, 64, 8), (2, 6
             (2, 127, 64, 2), (2, 128, 64, 4), (2, 128, 32, 1), (2, 128, 64, 8),
             (2, 86, 128, 4), (2, 85, 128, 8), (2, 83, 128, 16), (2, 114, 96, 3), (2, 113, 96, 6), (2, 44, 256, 8),
             (2, 42, 256, 32)]
-# (B, L, d, H, forced) on the shared-memory kernels: d / H = 64 always takes them; forced = the rt route switched off on
-# a shape it also accepts.  (2, 84, 128, 2), (2, 47, 256, 4), (2, 91, 64, 4) and (2, 42, 256, 8) are the largest L
-# their backward accepts: (4 L (d + 1) + H L (L + 1)) * 4 B <= 227 KB
-V1_CASES = [(3, 1, 64, 1, False), (3, 33, 128, 2, False), (2, 63, 64, 1, False), (2, 128, 64, 1, False),
-            (2, 31, 256, 4, False), (2, 84, 128, 2, False), (2, 47, 256, 4, False),
-            (3, 1, 32, 4, True), (3, 31, 64, 4, True), (3, 32, 96, 3, True), (2, 65, 32, 2, True), (2, 127, 32, 1, True),
-            (2, 128, 32, 1, True), (2, 63, 64, 8, True), (2, 91, 64, 4, True), (2, 42, 256, 8, True)]
-
+# (B, L, d, H) on the shared-memory kernels, the only route for d / H outside {8, 16, 32}.  (2, 84, 128, 2) and
+# (2, 47, 256, 4) are the largest L their backward accepts: (4 L (d + 1) + H L (L + 1)) * 4 B <= 227 KB
+V1_CASES = [(3, 1, 64, 1), (3, 33, 128, 2), (2, 63, 64, 1), (2, 128, 64, 1), (2, 31, 256, 4), (2, 84, 128, 2),
+            (2, 47, 256, 4),
+            (3, 17, 16, 4), (2, 100, 16, 4), (3, 7, 12, 1), (3, 40, 48, 4), (2, 128, 48, 1), (2, 64, 96, 4),
+            (2, 50, 96, 2), (2, 60, 128, 1), (2, 40, 256, 2)]
 
 def _check_attention(monkeypatch, B, L, d, H, live, route):
     from rechorus_b200 import ops
@@ -122,11 +120,8 @@ def test_causal_attention_rt_route_matches_float64(monkeypatch, B, L, d, H, live
 
 
 @pytest.mark.parametrize("live", [False, True])
-@pytest.mark.parametrize("B,L,d,H,forced", V1_CASES)
-def test_causal_attention_shared_memory_route_matches_float64(monkeypatch, B, L, d, H, forced, live):
-    from rechorus_b200 import ops
-    if forced:
-        monkeypatch.setattr(ops, "_ATTN_RT", False)
+@pytest.mark.parametrize("B,L,d,H", V1_CASES)
+def test_causal_attention_shared_memory_route_matches_float64(monkeypatch, B, L, d, H, live):
     _check_attention(monkeypatch, B, L, d, H, live, "v1")
 
 

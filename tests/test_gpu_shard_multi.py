@@ -29,8 +29,9 @@ def _free_port():
 def test_two_rank_sharded_step_matches_the_global_objective(exchange):
     cmd = [sys.executable, "-m", "torch.distributed.run", "--nnodes=1", "--nproc-per-node", "2", "--master-addr", "127.0.0.1",
            "--master-port", str(_free_port()), os.path.join(ROOT, "tools", "shard_bench.py"), "--check", "--n_items", "200000",
-           "--n_users", "50000", "--emb", "128", "--B", "512", "--K", "31", "--steps", "3", "--warmup", "1", "--optimizer", "SGD"]
-    env = dict(os.environ, B2R_SHARD_EXCHANGE=exchange, PYTHONPATH=ROOT)
+           "--n_users", "50000", "--emb", "128", "--B", "512", "--K", "31", "--steps", "3", "--warmup", "1", "--optimizer", "SGD",
+           "--exchange", exchange]
+    env = dict(os.environ, PYTHONPATH=ROOT)
     res = subprocess.run(cmd, capture_output=True, text=True, timeout=600, env=env)
     assert res.returncode == 0, (res.stdout + res.stderr)[-3000:]
     checks = [json.loads(ln) for ln in res.stdout.splitlines() if ln.startswith("{") and "check_max_abs_err" in ln]

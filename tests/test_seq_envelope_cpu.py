@@ -6,7 +6,7 @@ import types
 import pytest
 import torch
 
-LASTQ, V1 = 1, 2                     # B2R_SEQ_LAST_QUERY, B2R_SEQ_ATTN_V1
+LASTQ = 1                            # B2R_SEQ_LAST_QUERY
 
 
 @pytest.fixture(scope="module")
@@ -39,9 +39,9 @@ QUERY_CASES = [
     ((85, 128, 2, 1, 0), -3, "b2r_attention_bwd_live"),
     ((47, 256, 4, 1, 0), 0, None),
     ((48, 256, 4, 1, 0), -3, "b2r_attention_bwd_live"),
-    # the shared-memory kernels forced for every shape
-    ((128, 64, 4, 1, V1), -3, "b2r_attention_bwd_live"),
-    ((128, 32, 1, 1, V1), 0, None),
+    # every flag bit other than B2R_SEQ_LAST_QUERY is a bad argument
+    ((50, 64, 4, 1, 2), -1, "b2r_seq_train_check"),
+    ((50, 64, 4, 1, LASTQ | 2), -1, "b2r_seq_train_check"),
     # one 1-block SASRec: last-query block only, the position table has no limit of its own
     ((200, 64, 4, 0, LASTQ), 0, None),
     ((256, 64, 4, 0, LASTQ), 0, None),
@@ -112,11 +112,3 @@ def test_sasrec_outside_the_envelope_is_refused_at_construction(monkeypatch, lib
     assert f"history_max={hm}" in msg and f"emb_size={d}" in msg and f"num_heads={H}" in msg
     assert "b2r_" in msg                                     # the library's reason: which kernel, which limit
 
-
-def test_forcing_the_shared_memory_attention_kernels_narrows_the_envelope(monkeypatch, lib):
-    from rechorus_b200 import ops, plugin
-    monkeypatch.setattr(plugin, "_SASREC_LASTQ", True)
-    _build(64, 4, 2, 128)
-    monkeypatch.setattr(ops, "_ATTN_RT", False)
-    with pytest.raises(ValueError, match="b2r_attention_bwd_live"):
-        _build(64, 4, 2, 128)

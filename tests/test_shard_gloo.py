@@ -135,3 +135,15 @@ def test_bucket_by_owner_is_a_stable_partition():
     order, owner_sorted, rank, counts = _bucket_by_owner(owner, 4)
     assert order.tolist() == [1, 4, 5, 2, 6, 0, 3] and owner_sorted.tolist() == [0, 0, 0, 1, 1, 2, 2]
     assert rank.tolist() == [0, 1, 2, 0, 1, 0, 1] and counts.tolist() == [3, 2, 2, 0]
+
+
+def test_exchange_keyword_defaults_to_nccl_off_cuda_and_refuses_p2p_there():
+    from rechorus_b200.shard import ShardedBPRMF
+    cpu = torch.device("cpu")
+    assert ShardedBPRMF(N_USERS, N_ITEMS, D, cpu, backend=CpuStandIn(), optimizer="SGD").exchange == "nccl"
+    assert ShardedBPRMF(N_USERS, N_ITEMS, D, cpu, optimizer="SGD", exchange="nccl").exchange == "nccl"
+    for kw in ({"backend": CpuStandIn()}, {}):
+        with pytest.raises(ValueError, match="p2p"):
+            ShardedBPRMF(N_USERS, N_ITEMS, D, cpu, optimizer="SGD", exchange="p2p", **kw)
+    with pytest.raises(ValueError, match="exchange"):
+        ShardedBPRMF(N_USERS, N_ITEMS, D, cpu, backend=CpuStandIn(), optimizer="SGD", exchange="nvlink")

@@ -29,6 +29,8 @@ def main():
     ap.add_argument("--warmup", type=int, default=5)
     ap.add_argument("--optimizer", type=str, default="Adam")
     ap.add_argument("--check", action="store_true")
+    ap.add_argument("--exchange", choices=("p2p", "nccl"), default="p2p",
+                    help="p2p: kernels store into the peers' symmetric memory; nccl: the collective form")
     ap.add_argument("--torch_profile", action="store_true", help="print a torch.profiler kernel table for 3 steps (rank 0)")
     a = ap.parse_args()
     rank, world, local = int(os.environ.get("RANK", 0)), int(os.environ.get("WORLD_SIZE", 1)), int(os.environ.get("LOCAL_RANK", 0))
@@ -39,7 +41,8 @@ def main():
         dist.init_process_group("nccl", device_id=dev)
     from rechorus_b200 import ops
     from rechorus_b200.shard import ShardedBPRMF
-    m = ShardedBPRMF(a.n_users, a.n_items, a.emb, dev, optimizer=a.optimizer, lr=1e-3, init_std=0.1 if a.check else 0.01)
+    m = ShardedBPRMF(a.n_users, a.n_items, a.emb, dev, optimizer=a.optimizer, lr=1e-3, init_std=0.1 if a.check else 0.01,
+                     exchange=a.exchange)
     C = a.K + 1
     g = torch.Generator(device=dev).manual_seed(1234 + rank)
     pool = [(torch.randint(1, a.n_users, (a.B,), device=dev, generator=g),
