@@ -212,6 +212,10 @@ B2R_API int b2r_linear_fwd(const float* X, int ldx, const float* W, const float*
  * B2R_E_UNSUPPORTED outside that class. */
 B2R_API int b2r_linear_fwd_tc(const float* X, int ldx, const float* W, const float* bias, float* Y, int ldy,
                       int64_t M, int N, int K, int relu, b2r_stream_t stream);
+/* The route of the Linear forward for Y[M, N] = X[M, K] W^T: 1 when it runs on the tensor-core kernel above -- M >= 4096
+ * and the kernel's class, which also excludes N > 128 with K > 64 (W's tiles would not fit in one CTA's shared memory) --
+ * and 0 when it runs on the SGEMM (b2r_linear_fwd).  Alignment and leading dimensions aside.  Host only. */
+B2R_API int b2r_linear_fwd_uses_tc(int64_t M, int N, int K);
 /* general form: x_mask (same layout as X, may be NULL) zeroes X where x_mask <= 0 -- with X = dY, x_mask = the layer's
  * saved ReLU output and W = the transposed weight this is the input gradient dX = (dY * [y > 0]) W of a Linear layer */
 B2R_API int b2r_linear_tc(const float* X, int ldx, const float* x_mask, const float* W, const float* bias, float* Y,
@@ -486,6 +490,51 @@ B2R_API int b2r_topk_all_items(const float* Q, int ldq, const float* I, int64_t 
                                const int64_t* users, int B, const int64_t* clicked_ptr, const int64_t* clicked_items,
                                int64_t n_users, int k, int64_t* out_items, float* out_scores, int32_t* err_flag,
                                void* workspace, size_t workspace_bytes, b2r_stream_t stream);
+
+/* ------------------------------------------------------------------------------------------------
+ * NeuMF (models/general/NeuMF.py) against the whole catalogue: for the rows [b0, b1) of one evaluation batch of Bn
+ * users, out[(b - b0) * ld_out + c] = the score NeuMF's forward gives candidate column c of row b under test_all
+ * (column 0 the target, column c >= 1 item c) -- bit for bit, because the kernel runs the forward's own operations on the
+ * forward's own 64-row tiles of the flattened [Bn * n_items] candidate rows (the GMF dot of b2r_rowdot_fwd, the
+ * tensor-core Linear of b2r_linear_fwd_tc for every hidden layer, then the output layer's sequential fmaf chain).  The
+ * [Bn * n_items, 2d] concat input and the activations are never written.  Masking, ranking and top-k then run on the
+ * block through b2r_mask_clicked, b2r_gt_rank and b2r_topk_rows.
+ *
+ * b2r_neumf_score_rows_check: 0 when the shape is in the envelope, else B2R_E_UNSUPPORTED with b2r_last_error() naming
+ *   the refusing condition: d in {32, 64}, 1..B2R_NEUMF_MAX_LAYERS hidden layers, 4096 <= Bn * n_items < 2^31 (the
+ *   forward's tensor-core threshold), every hidden layer on the tensor-core kernel (b2r_linear_fwd_uses_tc) with at most
+ *   128 outputs at d = 32 and 64 at d = 64 (registers), and the resident weights plus operands within one CTA's shared memory.  Host only.
+ * b2r_neumf_window_rows: rows per window so that a [rows, n_items] float block stays within 32 MB (at least 1, at most
+ *   Bn).  Host only.
+ * b2r_neumf_score_rows: out-of-range user or target ids are clamped to row 0 and counted in err_flag.
+ * ---------------------------------------------------------------------------------------------- */
+#define B2R_NEUMF_MAX_LAYERS 4
+typedef struct {
+    const float*   mf_u;       /* [n_users, d]  mf_u_embeddings */
+    const float*   mf_i;       /* [n_items, d]  mf_i_embeddings */
+    const float*   mlp_u;      /* [n_users, d]  mlp_u_embeddings */
+    const float*   mlp_i;      /* [n_items, d]  mlp_i_embeddings */
+    int64_t        n_users;
+    int64_t        n_items;
+    int32_t        d;
+    int32_t        n_layers;
+    int32_t        widths[B2R_NEUMF_MAX_LAYERS];   /* hidden layer l: [widths[l], K_l] weight, K_0 = 2 d, K_l = widths[l - 1] */
+    const float*   W[B2R_NEUMF_MAX_LAYERS];        /* contiguous nn.Linear weights */
+    const float*   bias[B2R_NEUMF_MAX_LAYERS];     /* NULL: no bias */
+    const float*   w_out;      /* [d + widths[n_layers - 1]]  prediction.weight (GMF part first) */
+    const int64_t* users;      /* [Bn] */
+    const int64_t* targets;    /* [Bn]  column 0 of the candidate list */
+    int32_t        Bn;
+    int32_t        b0;
+    int32_t        b1;
+    int32_t        _pad;
+    float*         out;        /* [b1 - b0, ld_out] */
+    int64_t        ld_out;
+} b2r_neumf_rows;
+
+B2R_API int b2r_neumf_score_rows_check(int d, int n_layers, const int32_t* widths, int64_t Bn, int64_t n_items);
+B2R_API int b2r_neumf_window_rows(int64_t Bn, int64_t n_items);
+B2R_API int b2r_neumf_score_rows(const b2r_neumf_rows* rows, int32_t* err_flag, b2r_stream_t stream);
 
 /* ------------------------------------------------------------------------------------------------
  * Fused BPRMF forward + loss + query-side backward in one streaming pass: every candidate row is read from HBM once

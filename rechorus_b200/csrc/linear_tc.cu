@@ -13,29 +13,10 @@
 // shared memory in the K-major SWIZZLE_128B layout of wgmma_tf32.cuh, then fence.proxy.async + barrier, and the
 // warpgroup issues 3 * (K / 8) wgmmas.  The loads of the CTA's next tile are issued before the MMA wait, so they stay in
 // flight through the MMAs and the epilogue, which adds the bias, applies ReLU and stores Y straight from the accumulator.
-#include "common.cuh"
-#include "wgmma_tf32.cuh"
+#include "linear_tc.cuh"
 #include "dropout.cuh"
 
 namespace b2r {
-
-constexpr int TC_M = 64;           // rows per tile == wgmma M
-constexpr int TC_THREADS = 128;    // one warpgroup
-
-// round to the nearest TF32 value (10 explicit mantissa bits): the tensor core ignores the low 13 bits of what it is
-// given, so operands are pre-rounded here and arrive exactly representable
-__device__ __forceinline__ float tc_rn_tf32(float x) { return __uint_as_float((__float_as_uint(x) + 0x1000u) & 0xFFFFE000u); }
-
-// split 4 floats into hi = rn_tf32(x) and lo = rn_tf32(x - hi)  (|x - hi - lo| <= 2^-23 |x|), store both at the
-// swizzled chunk position
-__device__ __forceinline__ void tc_store_split(char* hi_base, char* lo_base, int row, int chunk, const float4& v) {
-    const uint32_t off = (uint32_t)row * 128u + (uint32_t)((chunk ^ (row & 7)) * 16);
-    float4 h, l;
-    h.x = tc_rn_tf32(v.x); h.y = tc_rn_tf32(v.y); h.z = tc_rn_tf32(v.z); h.w = tc_rn_tf32(v.w);
-    l.x = tc_rn_tf32(v.x - h.x); l.y = tc_rn_tf32(v.y - h.y); l.z = tc_rn_tf32(v.z - h.z); l.w = tc_rn_tf32(v.w - h.w);
-    *reinterpret_cast<float4*>(hi_base + off) = h;
-    *reinterpret_cast<float4*>(lo_base + off) = l;
-}
 
 // dynamic shared memory (1024-byte aligned): A_hi[KS][64*128B] A_lo[...] B_hi[KS][NW*128B] B_lo[...]; NW >= N is the
 // wgmma width, W's rows N..NW-1 are zero and their output columns are not stored.  DROP: dropout (dropout.cuh) after
@@ -104,18 +85,7 @@ k_linear_tc(const float* __restrict__ X, int ldx, const float* __restrict__ amas
         asm volatile("fence.proxy.async.shared::cta;" ::: "memory");      // generic-proxy stores -> async proxy (wgmma)
         __syncthreads();
         wg_fence();
-#pragma unroll
-        for (int prod = 0; prod < 3; ++prod) {                  // hi*hi, hi*lo, lo*hi
-            const char* Ab = (prod < 2) ? A_hi : A_lo;
-            const char* Bb = (prod & 1) ? B_lo : B_hi;
-#pragma unroll
-            for (int s = 0; s < KS; ++s) {
-#pragma unroll
-                for (int k = 0; k < 4; ++k)                     // 4 MMAs of K = 8 floats (32 bytes) per slab
-                    wgmma_tf32<NW>(acc, wg_desc(wg_smem_u32(Ab + s * a_slab) + k * 32),
-                                   wg_desc(wg_smem_u32(Bb + s * b_slab) + k * 32), (prod | s | k) != 0);
-            }
-        }
+        tc_mma_3x<KS, NW>(acc, A_hi, A_lo, B_hi, B_lo);
         wg_commit();
         if (tile + (int)gridDim.x < ntiles) issue_loads(tile + (int)gridDim.x);
         wg_wait_all();
@@ -183,12 +153,16 @@ static int launch_linear_tc_ks(const float* X, int ldx, const float* x_mask, con
     return set_error(B2R_E_UNSUPPORTED, "b2r_linear_tc: N=%d with K=%d exceeds the shared memory of one CTA", N, KS * 32);
 }
 
+bool linear_tc_shape(int64_t M, int N, int K) {
+    return K % 32 == 0 && K >= 32 && K <= 128 && N % 16 == 0 && N >= 16 && N <= 256 && M > 0 && M <= 0x7fffffff &&
+           !(N > 128 && K > 64);
+}
+
 template <bool DROP>
 static int linear_tc(const float* X, int ldx, const float* x_mask, const float* W, const float* bias, float* Y, int ldy,
                      int64_t M, int N, int K, int relu, const DropK& dk, cudaStream_t s) {
     B2R_REQUIRE(X && W && Y, B2R_E_BADARG, "b2r_linear_fwd_tc: null pointer");
-    if (!(K % 32 == 0 && K >= 32 && K <= 128 && N % 16 == 0 && N >= 16 && N <= 256 && M > 0 && M <= 0x7fffffff &&
-          ldx % 4 == 0 && ldy % 4 == 0 && aligned16(X) && aligned16(W) && aligned16(Y) &&
+    if (!(linear_tc_shape(M, N, K) && ldx % 4 == 0 && ldy % 4 == 0 && aligned16(X) && aligned16(W) && aligned16(Y) &&
           (x_mask == nullptr || aligned16(x_mask))))
         return set_error(B2R_E_UNSUPPORTED, "b2r_linear_fwd_tc: shape M=%lld N=%d K=%d ldx=%d ldy=%d outside the kernel's class",
                          (long long)M, N, K, ldx, ldy);
@@ -203,6 +177,10 @@ static int linear_tc(const float* X, int ldx, const float* x_mask, const float* 
 }  // namespace b2r
 
 using namespace b2r;
+
+extern "C" int b2r_linear_fwd_uses_tc(int64_t M, int N, int K) {
+    return M >= kTcMinRows && linear_tc_shape(M, N, K) ? 1 : 0;
+}
 
 // returns B2R_E_UNSUPPORTED for shapes outside the tensor-core kernel's class (callers fall back to b2r_linear_fwd)
 extern "C" int b2r_linear_fwd_tc(const float* X, int ldx, const float* W, const float* bias, float* Y, int ldy, int64_t M,

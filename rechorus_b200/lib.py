@@ -41,6 +41,19 @@ class Dropout(C.Structure):
                 ("L", C.c_int32)]
 
 
+NEUMF_MAX_LAYERS = 4                        # B2R_NEUMF_MAX_LAYERS
+
+
+class NeumfRows(C.Structure):
+    """b2r_neumf_rows (include/b200rec.h)"""
+    _fields_ = [("mf_u", C.c_void_p), ("mf_i", C.c_void_p), ("mlp_u", C.c_void_p), ("mlp_i", C.c_void_p),
+                ("n_users", C.c_int64), ("n_items", C.c_int64), ("d", C.c_int32), ("n_layers", C.c_int32),
+                ("widths", C.c_int32 * NEUMF_MAX_LAYERS), ("W", C.c_void_p * NEUMF_MAX_LAYERS),
+                ("bias", C.c_void_p * NEUMF_MAX_LAYERS), ("w_out", C.c_void_p), ("users", C.c_void_p),
+                ("targets", C.c_void_p), ("Bn", C.c_int32), ("b0", C.c_int32), ("b1", C.c_int32), ("_pad", C.c_int32),
+                ("out", C.c_void_p), ("ld_out", C.c_int64)]
+
+
 OPT_SGD, OPT_ADAM, OPT_ADAGRAD = 0, 1, 2
 SEQ_LAST_QUERY = 1                          # b2r_seq_train_check flag
 PROF_SCORE_FWD, PROF_SCORE_BWDQ, PROF_SEGMENT_I, PROF_SEGMENT_U, PROF_PLAN_I, PROF_LOSS = range(6)
@@ -85,6 +98,7 @@ SIGNATURES = {
                                  C.c_int, C.c_int, C.c_int, C.c_void_p]),
     "b2r_linear_fwd_tc": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int64,
                                     C.c_int, C.c_int, C.c_int, C.c_void_p]),
+    "b2r_linear_fwd_uses_tc": (C.c_int, [C.c_int64, C.c_int, C.c_int]),
     "b2r_linear_tc": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int64,
                                 C.c_int, C.c_int, C.c_int, C.c_void_p]),
     "b2r_linear_bwd_input": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int,
@@ -149,6 +163,9 @@ SIGNATURES = {
     "b2r_topk_all_items": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p, C.c_int64, C.c_int, C.c_void_p, C.c_void_p,
                                      C.c_int, C.c_void_p, C.c_void_p, C.c_int64, C.c_int, C.c_void_p, C.c_void_p,
                                      C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p]),
+    "b2r_neumf_score_rows_check": (C.c_int, [C.c_int, C.c_int, C.c_void_p, C.c_int64, C.c_int64]),
+    "b2r_neumf_window_rows": (C.c_int, [C.c_int64, C.c_int64]),
+    "b2r_neumf_score_rows": (C.c_int, [C.POINTER(NeumfRows), C.c_void_p, C.c_void_p]),
     "b2r_adam_exact_advance": (C.c_int, [C.c_void_p, C.c_int64, C.c_int64, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p,
                                          C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p]),
     "b2r_sample_negatives": (C.c_int, [C.c_void_p, C.c_int64, C.c_int, C.c_void_p, C.c_void_p, C.c_int64, C.c_int64,

@@ -367,6 +367,70 @@ def topk_all_items(q: torch.Tensor, table: torch.Tensor, target: torch.Tensor, u
     return items, scores
 
 
+def neumf_all_items_error(d: int, layers: Sequence[int], Bn: int, n_items: int) -> Optional[str]:
+    """None when NeuMF's test_all scores of a batch of Bn rows can come from neumf_score_rows (d in {32, 64}, at least
+    4096 candidate rows, every hidden layer on the forward's tensor-core Linear, the fused CTA within shared memory), else
+    why not (b2r_neumf_score_rows_check; host only)"""
+    layers = [int(w) for w in layers]
+    if not 1 <= len(layers) <= _lib.NEUMF_MAX_LAYERS:
+        return f"{len(layers)} hidden layers, the fused scorer takes 1..{_lib.NEUMF_MAX_LAYERS}"
+    widths = (C.c_int32 * len(layers))(*layers)
+    L = _lib.load()
+    if L.b2r_neumf_score_rows_check(int(d), len(layers), widths, int(Bn), int(n_items)) == 0:
+        return None
+    return L.b2r_last_error().decode("utf-8", "replace")
+
+
+def neumf_window_rows(Bn: int, n_items: int) -> int:
+    """rows of one neumf_score_rows window: a [rows, n_items] float32 block within 32 MB, at least one row"""
+    return int(_lib.load().b2r_neumf_window_rows(int(Bn), int(n_items)))
+
+
+def neumf_score_rows(mf_u: torch.Tensor, mf_i: torch.Tensor, mlp_u: torch.Tensor, mlp_i: torch.Tensor,
+                     mlp: Sequence[Tuple[torch.Tensor, Optional[torch.Tensor]]], w_out: torch.Tensor, users: torch.Tensor,
+                     targets: torch.Tensor, b0: int, b1: int, out: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """Rows [b0, b1) of NeuMF's test_all scores for one evaluation batch (users [Bn], targets [Bn]): the [b1 - b0,
+    n_items] block NeuMF's forward gives on the candidate list [target | arange(1, n_items)], bit for bit (column 0 the
+    target, column j >= 1 item j), without the [Bn * n_items, 2d] concat input (b2r_neumf_score_rows).  mlp: the hidden
+    layers' (weight [N, K], bias [N] or None); w_out: prediction.weight [1, d + last].  Raises B200RecError for shapes
+    outside neumf_all_items_error's envelope; out-of-range user / target ids make check_ids raise IndexError."""
+    _need_cuda(mf_u, mf_i, mlp_u, mlp_i, w_out, users, targets)
+    mf_u, mf_i, mlp_u, mlp_i = (_f32c(t, n) for t, n in ((mf_u, "mf_u"), (mf_i, "mf_i"), (mlp_u, "mlp_u"), (mlp_i, "mlp_i")))
+    w_out = _f32c(w_out.reshape(-1), "w_out")
+    users, targets = _i64c(users.reshape(-1), "users"), _i64c(targets.reshape(-1), "targets")
+    n_users, d = mf_u.shape
+    n_items = mf_i.shape[0]
+    Bn = users.numel()
+    if targets.numel() != Bn or mlp_u.shape != mf_u.shape or mlp_i.shape != mf_i.shape or mf_i.shape[1] != d:
+        raise ValueError("neumf_score_rows: tables [n_users, d] / [n_items, d], users and targets [Bn]")
+    if not 0 <= b0 < b1 <= Bn:
+        raise ValueError(f"neumf_score_rows: window [{b0}, {b1}) outside the batch of {Bn} rows")
+    if not 1 <= len(mlp) <= _lib.NEUMF_MAX_LAYERS:
+        raise ValueError(f"neumf_score_rows: {len(mlp)} hidden layers, the fused scorer takes 1..{_lib.NEUMF_MAX_LAYERS}")
+    Ws = [_f32c(W, f"W{l}") for l, (W, _) in enumerate(mlp)]
+    bs = [None if b is None else _f32c(b, f"bias{l}") for l, (_, b) in enumerate(mlp)]
+    for l, (W, b) in enumerate(zip(Ws, bs)):
+        K = 2 * d if l == 0 else Ws[l - 1].shape[0]
+        if W.dim() != 2 or W.shape[1] != K or (b is not None and b.numel() != W.shape[0]):
+            raise ValueError(f"neumf_score_rows: hidden layer {l} must be a [N, {K}] weight with an [N] bias")
+    if w_out.numel() != d + Ws[-1].shape[0]:
+        raise ValueError("neumf_score_rows: w_out must hold d + the last hidden width")
+    if out is None:
+        out = torch.empty((b1 - b0, n_items), dtype=torch.float32, device=mf_u.device)
+    elif out.dtype != torch.float32 or out.dim() != 2 or out.shape != (b1 - b0, n_items) or out.stride(1) != 1:
+        raise ValueError("neumf_score_rows: out must be float32 [b1 - b0, n_items] with contiguous rows")
+    a = _lib.NeumfRows()
+    a.mf_u, a.mf_i, a.mlp_u, a.mlp_i = _p(mf_u), _p(mf_i), _p(mlp_u), _p(mlp_i)
+    a.n_users, a.n_items, a.d, a.n_layers = n_users, n_items, d, len(Ws)
+    for l, (W, b) in enumerate(zip(Ws, bs)):
+        a.widths[l], a.W[l], a.bias[l] = W.shape[0], _p(W), _p(b)
+    a.w_out, a.users, a.targets = _p(w_out), _p(users), _p(targets)
+    a.Bn, a.b0, a.b1 = Bn, int(b0), int(b1)
+    a.out, a.ld_out = _p(out), out.stride(0)
+    _lib.check(_lib.load().b2r_neumf_score_rows(C.byref(a), _p(err_flag(mf_u.device)), _stream()), "b2r_neumf_score_rows")
+    return out
+
+
 class DeviceNegativeSampler:
     """Groundwork for SURVEY.md §8 f3: models/BaseModel.py:206-214 on the device.  Holds the training clicks as a CSR
     on the GPU and draws ``num_neg`` non-clicked items per training row with b2r_sample_negatives.  Same distribution
@@ -937,6 +1001,12 @@ def linear_fwd(x: torch.Tensor, W: torch.Tensor, bias: Optional[torch.Tensor], r
     return y
 
 
+def linear_fwd_uses_tc(M: int, N: int, K: int) -> bool:
+    """whether the Linear forward of X[M, K] W^T with W [N, K] runs on the tensor-core kernel (b2r_linear_fwd_uses_tc)
+    rather than the SGEMM -- the library's one copy of that decision"""
+    return bool(_lib.load().b2r_linear_fwd_uses_tc(int(M), int(N), int(K)))
+
+
 def linear_fwd_tc(x: torch.Tensor, W: torch.Tensor, bias: Optional[torch.Tensor], relu: bool, strict: bool = True):
     """same as linear_fwd on the tensor cores (wgmma, TF32 hi/lo split, fp32-class accuracy); for shapes outside the
     kernel's class it raises (strict) or returns None"""
@@ -1103,7 +1173,7 @@ class _Linear(torch.autograd.Function):
         N, K = W.shape
         # a long batch dimension (M >= 4096) runs on the tensor cores (csrc/linear_tc.cu: wgmma, TF32 hi/lo split,
         # 3 products, fp32-class accuracy checked in tests/test_gpu_tc.py); linear_bwd picks dX and dW the same way
-        tc = x2.shape[0] >= 4096 and K % 32 == 0 and K <= 128 and N % 16 == 0 and N <= 256
+        tc = linear_fwd_uses_tc(x2.shape[0], N, K)
         if drop is not None:
             if not relu:
                 raise ValueError("fused dropout follows a ReLU (its backward reads the mask off the saved output)")

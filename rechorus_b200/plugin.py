@@ -137,9 +137,7 @@ class _KernelModelMixin:
         ``clicked`` (ops.ClickedSets, test_all only) names those pairs instead as the clicked items of each row's user;
         a dot-product model then needs only column 0 of feed_dict["item_id"]."""
         with torch.no_grad():
-            opt = self.__dict__.get("_b2r_optimizer")
-            if getattr(opt, "exact_dense", False) and not self.training:
-                opt.flush()                     # exact dense-Adam mode: ranks must see rows advanced through skipped steps
+            self._flush_exact()
             item_id = feed_dict["item_id"]
             test_all = bool(getattr(self, "test_all", 0))
             if clicked is not None and test_all and self.has_query_rows():
@@ -159,6 +157,11 @@ class _KernelModelMixin:
                 pred[mask_row, mask_item] = float("-inf")
             return ops.gt_rank(pred)
 
+    def _flush_exact(self) -> None:
+        opt = self.__dict__.get("_b2r_optimizer")
+        if getattr(opt, "exact_dense", False) and not self.training:
+            opt.flush()                     # exact dense-Adam mode: ranks and lists must see rows advanced through skipped steps
+
     def has_query_rows(self) -> bool:
         """whether this model scores candidates as dot products with item-table rows (query_rows is overridden)"""
         return type(self).query_rows is not _KernelModelMixin.query_rows
@@ -170,9 +173,7 @@ class _KernelModelMixin:
         ``clicked`` (ops.ClickedSets) masked to -inf (BaseRunner.py:244-251); column 0 of feed_dict["item_id"] is the
         target and a dot-product model needs no other column (ops.topk_all_items scores the catalogue itself)."""
         with torch.no_grad():
-            opt = self.__dict__.get("_b2r_optimizer")
-            if getattr(opt, "exact_dense", False) and not self.training:
-                opt.flush()                     # exact dense-Adam mode: lists must see rows advanced through skipped steps
+            self._flush_exact()
             item_id = feed_dict["item_id"]
             test_all = bool(getattr(self, "test_all", 0))
             if test_all and clicked is None:
@@ -321,6 +322,65 @@ class NeuMFKernels(_KernelModelMixin):
             h = ops.linear(h, layer.weight, layer.bias, relu=True, drop=drop)
         pred = pred + ops.linear(h, w_out[:, d:], None, relu=False).view(B, C)
         return {"prediction": pred.view(feed_dict["batch_size"], -1)}
+
+    # test_all without the [Bn * n_items, 2d] concat input: the forward's scores are produced window by window of batch
+    # rows by ops.neumf_score_rows, bit for bit, and masked / ranked / selected by the same kernels as the forward's
+    # matrix would be, so ranks and lists are the materialised route's.  Outside the envelope (training mode, no clicked
+    # sets, a batch below the forward's tensor-core threshold, a layer the forward runs on the SGEMM, a CTA that would not
+    # fit) the materialised route runs as before.
+    def _all_items_fused(self, feed_dict, clicked, mask_row=None) -> bool:
+        if self.training or clicked is None or mask_row is not None or not getattr(self, "test_all", 0):
+            return False
+        if feed_dict["item_id"].shape[1] != self.item_num:
+            return False                    # the materialised route reports the malformed candidate list
+        widths = [layer.weight.shape[0] for layer in self.mlp]
+        return ops.neumf_all_items_error(self.emb_size, widths, feed_dict["user_id"].numel(), self.item_num) is None
+
+    def _all_items_windows(self, feed_dict):
+        """yields (b0, b1, scores [b1 - b0, n_items]) over the batch; the score buffer is reused by the next window"""
+        users = feed_dict["user_id"]
+        target = feed_dict["item_id"][:, 0]
+        Bn = users.numel()
+        rows = ops.neumf_window_rows(Bn, self.item_num)
+        buf = torch.empty((rows, self.item_num), dtype=torch.float32, device=users.device)
+        mlp = [(layer.weight, layer.bias) for layer in self.mlp]
+        for b0 in range(0, Bn, rows):
+            b1 = min(Bn, b0 + rows)
+            yield b0, b1, ops.neumf_score_rows(self.mf_u_embeddings.weight, self.mf_i_embeddings.weight,
+                                               self.mlp_u_embeddings.weight, self.mlp_i_embeddings.weight, mlp,
+                                               self.prediction.weight, users, target, b0, b1, out=buf[:b1 - b0])
+
+    def eval_ranks(self, feed_dict: dict, mask_row=None, mask_item=None, clicked=None) -> torch.Tensor:
+        """_KernelModelMixin.eval_ranks; inside the fused route's envelope only column 0 (the target) of
+        feed_dict["item_id"] is read: the other columns must be the test_all list arange(1, n_items), as every
+        collate_batch / device_eval_batches batch under test_all has them, since the scorer takes item j for column j."""
+        if not self._all_items_fused(feed_dict, clicked, mask_row):
+            return super().eval_ranks(feed_dict, mask_row, mask_item, clicked)
+        with torch.no_grad():
+            self._flush_exact()
+            users = feed_dict["user_id"]
+            rank = torch.empty(users.numel(), dtype=torch.int64, device=users.device)
+            for b0, b1, scores in self._all_items_windows(feed_dict):
+                rank[b0:b1] = ops.gt_rank(ops.mask_clicked(scores, users[b0:b1], clicked))
+            return rank
+
+    def recommend(self, feed_dict: dict, k: int, clicked=None):
+        """_KernelModelMixin.recommend; inside the fused route's envelope only column 0 of feed_dict["item_id"] is
+        read, as in eval_ranks"""
+        if not self._all_items_fused(feed_dict, clicked):
+            return super().recommend(feed_dict, k, clicked)
+        with torch.no_grad():
+            self._flush_exact()
+            users, target = feed_dict["user_id"], feed_dict["item_id"][:, 0]
+            kk = min(ops._topk_k(k), self.item_num)
+            items = torch.empty((users.numel(), kk), dtype=torch.int64, device=users.device)
+            scores = torch.empty((users.numel(), kk), dtype=torch.float32, device=users.device)
+            for b0, b1, block in self._all_items_windows(feed_dict):
+                cols, vals = ops.topk_rows(ops.mask_clicked(block, users[b0:b1], clicked), k)
+                # column 0 is the target, column j >= 1 item j (the candidate list [target | arange(1, n_items)])
+                items[b0:b1] = torch.where(cols == 0, target[b0:b1].view(-1, 1), cols)
+                scores[b0:b1] = vals
+            return items, scores
 
 
 class _AttentionParams(nn.Module):

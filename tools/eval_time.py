@@ -10,8 +10,10 @@ built on the device, ranks and histogram on the device), in one process, alterna
                      route materialises [rows, n_items] predictions and masks them in a Python loop, so it is timed on a
                      sample of the rows (--buffer 0: feed dicts built per batch; no DataLoader workers, whose
                      [256, n_items] int64 batches would pass through shared memory) and scaled per row; the output says so.
+  NeuMF test_all     the fused route against the materialised one at 100k items and the fused route at 1M items
+                     (tools/neumf_all_time.py; CUDA events around NeuMF.eval_ranks on one batch of 256 users).
 
-Every time is a host clock around the evaluate call followed by torch.cuda.synchronize().  The device route's first call
+Every other time is a host clock around the evaluate call followed by torch.cuda.synchronize().  The device route's first call
 also uploads the phase's columns and builds the clicked-item CSR; it is reported on its own as "first_call_s".  Both routes'
 metrics are compared on the rows both evaluated.  One JSON line per case, then one with the card's name, power limit and
 max SM clock read in the same run.
@@ -145,7 +147,8 @@ def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--reps", type=int, default=3)
     ap.add_argument("--num_workers", type=int, default=5, help="the host route's DataLoader workers (runner default 5)")
-    ap.add_argument("--cases", nargs="+", default=list(CASES))
+    ap.add_argument("--cases", nargs="*", default=list(CASES))
+    ap.add_argument("--skip-neumf", action="store_true", help="skip the NeuMF test_all cases")
     a = ap.parse_args()
     if not torch.cuda.is_available():
         raise SystemExit("eval_time.py measures on a CUDA device; none found")
@@ -153,6 +156,10 @@ def main():
     for name in a.cases:
         print(json.dumps(run_case(name, a.reps, a.num_workers)), flush=True)
         torch.cuda.empty_cache()
+    if not a.skip_neumf:
+        from neumf_all_time import neumf_all_items
+        for ln in neumf_all_items("ranks", a.reps):
+            print(json.dumps(ln), flush=True)
     print(json.dumps(card()), flush=True)
 
 

@@ -11,6 +11,8 @@
              reference's host route (predict with the host mask loop, Python sort of every row, CSV write).  The host route
              runs on a 500-user subset and is scaled per row to 100k rows; the output says so.  Host clocks around work
              that ends in a device synchronise.
+  neumf      NeuMF under test_all: NeuMF.recommend(k=100) on the fused route against the materialised one at 100k items,
+             the fused route at 1M items (tools/neumf_all_time.py).
 
   split      device time per kernel of one topk_all_items and one rank_all_items call (torch.profiler, CUDA activities),
              in a pass of its own after the timed ones.
@@ -202,12 +204,16 @@ def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--reps", type=int, default=3)
     ap.add_argument("--skip-runner", action="store_true")
+    ap.add_argument("--only-neumf", action="store_true", help="run the NeuMF test_all cases alone")
     a = ap.parse_args()
     if not torch.cuda.is_available():
         raise SystemExit("rec_time.py measures on a CUDA device; none found")
+    from neumf_all_time import neumf_all_items
     from seq_batches_time import card
-    for part in (all_items, rows) + (() if a.skip_runner else (runner_route,)) + (kernel_split,):
-        for ln in part(a.reps) if part in (all_items, rows) else part():
+    neumf = lambda reps: neumf_all_items("lists", reps)
+    parts = (neumf,) if a.only_neumf else (all_items, rows) + (() if a.skip_runner else (runner_route,)) + (neumf, kernel_split)
+    for part in parts:
+        for ln in part(a.reps) if part in (all_items, rows, neumf) else part():
             print(json.dumps(ln), flush=True)
     print(json.dumps(card()), flush=True)
 
