@@ -492,6 +492,48 @@ B2R_API int b2r_topk_all_items(const float* Q, int ldq, const float* I, int64_t 
                                void* workspace, size_t workspace_bytes, b2r_stream_t stream);
 
 /* ------------------------------------------------------------------------------------------------
+ * Impression evaluation (row f4): ImpressionRunner.evaluate (helpers/ImpressionRunner.py:135-171) for the
+ * non-test_all branch on the device, batch by batch, without feed dicts or a host copy of the predictions.
+ *
+ * b2r_collate_impression: rows [start, start + Bn) of an evaluation phase as ImpressionModel.Dataset builds them
+ *                     (models/BaseImpressionModel.py:152-184): out_uid int64 [Bn] = users[start + t], out_iid int64
+ *                     [Bn, mp + mn] = [pos[:mp] | 0 up to mp | neg[:mn] | 0 up to mn].  The lists are a CSR over the
+ *                     phase's rows: row r's positives at pos_items[pos_ptr[r] .. pos_ptr[r + 1]), its negatives at
+ *                     neg_items[neg_ptr[r] .. neg_ptr[r + 1]); only the first mp / mn entries are read.  A user outside
+ *                     [0, n_users) is clamped to 0 and counted in err_flag.
+ * b2r_impression_metrics: adds the per-row NDCG@k, MAP@k and HR@k of one batch's predictions pred [Bn, C] (row stride ld,
+ *                     C = mp + mn) into acc float64 [3 * nk]: acc[i] += sum of NDCG@topk[i], acc[nk + i] += sum of MAP@..,
+ *                     acc[2 nk + i] += sum of HR@..; the caller divides by the row count.  pos_num / neg_num int64 [Bn]
+ *                     are the raw data columns of the batch's rows; topk is a HOST array of 1 <= nk <= 16 cut-offs.
+ *                     The contract, per row, with P = min(pos_num, mp), Q = min(neg_num, C - mp), W = P + Q:
+ *                       - columns [0, P) and [mp, mp + Q) are valid; every other column's prediction is -inf;
+ *                       - key[c] = (double)pred[c] - 1e-6 for c < mp, (double)pred[c] otherwise;
+ *                       - order: key descending, ties by column ascending, NaN after everything (NaNs by column);
+ *                         +0.0 and -0.0 are equal.  That is NumPy's stable argsort of -key;
+ *                       - r_j = the number of columns before valid positive j (j < P); only r_j < W count, and Pm is
+ *                         how many do.  With m_j = 1 + #{j' : r_j' < r_j}:
+ *                         DCG@k = sum_{r_j < k} 1 / log2(r_j + 2), IDCG@k = sum_{t < min(Pm, k)} 1 / log2(t + 2)
+ *                         (1 when 0), NDCG@k = DCG / IDCG;  MAP@k = sum_{r_j < k} m_j / (r_j + 1) / min(max(Pm, 1), k);
+ *                         HR@k = 1 if some r_j < k, else 0.
+ *                     One warp per row ranks every valid positive by counting over the row's keys in shared memory.
+ *                     Sums run in a fixed order: lanes, then the rows of a CTA (a CTA holds a number of rows fixed
+ *                     by C), then the CTAs in index order in the last CTA to finish -- so the result does not depend
+ *                     on scheduling and two calls give identical bits.  Workspace:
+ *                     b2r_impression_metrics_workspace_bytes(Bn, C, nk); its first 16 bytes are a counter that must be
+ *                     zero before the first call (every call leaves it zero).  C above what one warp's shared memory
+ *                     holds (about 19,000) or nk > 16 is B2R_E_UNSUPPORTED.
+ * ---------------------------------------------------------------------------------------------- */
+#define B2R_IMPRESSION_MAX_TOPK 16
+B2R_API int b2r_collate_impression(const int64_t* users, const int64_t* pos_ptr, const int64_t* pos_items,
+                                   const int64_t* neg_ptr, const int64_t* neg_items, int64_t n_users, int64_t start,
+                                   int Bn, int mp, int mn, int64_t* out_uid, int64_t* out_iid, int32_t* err_flag,
+                                   b2r_stream_t stream);
+B2R_API size_t b2r_impression_metrics_workspace_bytes(int Bn, int C, int nk);
+B2R_API int b2r_impression_metrics(const float* pred, int64_t ld, int Bn, int C, int mp, const int64_t* pos_num,
+                                   const int64_t* neg_num, const int* topk, int nk, double* acc, void* workspace,
+                                   size_t workspace_bytes, b2r_stream_t stream);
+
+/* ------------------------------------------------------------------------------------------------
  * NeuMF (models/general/NeuMF.py) against the whole catalogue: for the rows [b0, b1) of one evaluation batch of Bn
  * users, out[(b - b0) * ld_out + c] = the score NeuMF's forward gives candidate column c of row b under test_all
  * (column 0 the target, column c >= 1 item c) -- bit for bit, because the kernel runs the forward's own operations on the

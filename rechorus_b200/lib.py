@@ -54,6 +54,8 @@ class NeumfRows(C.Structure):
                 ("out", C.c_void_p), ("ld_out", C.c_int64)]
 
 
+IMPRESSION_MAX_TOPK = 16                    # B2R_IMPRESSION_MAX_TOPK
+
 OPT_SGD, OPT_ADAM, OPT_ADAGRAD = 0, 1, 2
 SEQ_LAST_QUERY = 1                          # b2r_seq_train_check flag
 PROF_SCORE_FWD, PROF_SCORE_BWDQ, PROF_SEGMENT_I, PROF_SEGMENT_U, PROF_PLAN_I, PROF_LOSS = range(6)
@@ -163,6 +165,11 @@ SIGNATURES = {
     "b2r_topk_all_items": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p, C.c_int64, C.c_int, C.c_void_p, C.c_void_p,
                                      C.c_int, C.c_void_p, C.c_void_p, C.c_int64, C.c_int, C.c_void_p, C.c_void_p,
                                      C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p]),
+    "b2r_collate_impression": (C.c_int, [C.c_void_p] * 5 + [C.c_int64, C.c_int64, C.c_int, C.c_int, C.c_int,
+                                                            C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "b2r_impression_metrics_workspace_bytes": (C.c_size_t, [C.c_int, C.c_int, C.c_int]),
+    "b2r_impression_metrics": (C.c_int, [C.c_void_p, C.c_int64, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p,
+                                         C.POINTER(C.c_int), C.c_int, C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p]),
     "b2r_neumf_score_rows_check": (C.c_int, [C.c_int, C.c_int, C.c_void_p, C.c_int64, C.c_int64]),
     "b2r_neumf_window_rows": (C.c_int, [C.c_int64, C.c_int64]),
     "b2r_neumf_score_rows": (C.c_int, [C.POINTER(NeumfRows), C.c_void_p, C.c_void_p]),

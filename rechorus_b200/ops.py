@@ -545,6 +545,79 @@ def collate_history(users: torch.Tensor, positions: torch.Tensor, his_ptr: torch
                                                _p(out_len), _p(err_flag(users.device)), _stream()), "b2r_collate_history")
 
 
+def list_csr(lists, width: int):
+    """Ragged per-row lists (e.g. an impression phase's ``pos_items`` column) cut to their first ``width`` entries, as a
+    CSR over the rows: ptr int64 [N + 1] and items int64 (at least one slot).  NumPy arrays; one pass over the lists."""
+    import itertools
+
+    import numpy as np
+    width = int(width)
+    lens = np.fromiter((min(len(x), width) for x in lists), dtype=np.int64, count=len(lists))
+    ptr = np.zeros(len(lists) + 1, dtype=np.int64)
+    np.cumsum(lens, out=ptr[1:])
+    items = np.fromiter(itertools.chain.from_iterable(x[:width] for x in lists), dtype=np.int64, count=int(ptr[-1]))
+    return ptr, (items if len(items) else np.zeros(1, dtype=np.int64))
+
+
+def collate_impression(users: torch.Tensor, pos_ptr: torch.Tensor, pos_items: torch.Tensor, neg_ptr: torch.Tensor,
+                       neg_items: torch.Tensor, n_users: int, start: int, Bn: int, mp: int, mn: int, out_uid: torch.Tensor,
+                       out_iid: torch.Tensor) -> None:
+    """b2r_collate_impression: rows [start, start + Bn) of an impression evaluation phase as ImpressionModel.Dataset's
+    collate_batch builds them (models/BaseImpressionModel.py:152-184): out_uid[t] = users[start + t], out_iid[t] =
+    [pos[:mp] | 0-pad | neg[:mn] | 0-pad], the lists read from the CSRs (pos_ptr, pos_items) / (neg_ptr, neg_items) over
+    the phase's rows (list_csr).  A user outside [0, n_users) makes check_ids raise IndexError."""
+    _need_cuda(users, pos_ptr, pos_items, neg_ptr, neg_items, out_uid, out_iid)
+    for t in (users, pos_ptr, pos_items, neg_ptr, neg_items, out_uid, out_iid):
+        if t.dtype != torch.int64 or not t.is_contiguous():
+            raise TypeError("collate_impression: contiguous int64 tensors expected")
+    N = users.numel()
+    if not 0 <= start <= start + Bn <= N or pos_ptr.numel() != N + 1 or neg_ptr.numel() != N + 1:
+        raise ValueError("collate_impression: rows outside the phase, or CSRs that do not cover its rows")
+    if out_iid.dim() != 2 or out_iid.shape[1] != mp + mn or out_iid.shape[0] < Bn or out_uid.numel() < Bn:
+        raise ValueError("collate_impression: output buffers do not fit the batch")
+    _lib.check(_lib.load().b2r_collate_impression(_p(users), _p(pos_ptr), _p(pos_items), _p(neg_ptr), _p(neg_items),
+                                                  int(n_users), int(start), int(Bn), int(mp), int(mn), _p(out_uid),
+                                                  _p(out_iid), _p(err_flag(users.device)), _stream()),
+               "b2r_collate_impression")
+
+
+_imp_ws = {}
+
+
+def impression_metrics(pred: torch.Tensor, pos_num: torch.Tensor, neg_num: torch.Tensor, mp: int, topk: Sequence[int],
+                       acc: torch.Tensor) -> torch.Tensor:
+    """b2r_impression_metrics: adds the per-row NDCG@k, MAP@k and HR@k sums of one batch of impression predictions
+    pred [Bn, mp + mn] into acc float64 [3 * len(topk)] (NDCG for every k, then MAP, then HR), the metrics of
+    ImpressionRunner.evaluate (helpers/ImpressionRunner.py:135-171, :74-133) as include/b200rec.h restates them.
+    pos_num / neg_num: the batch rows' raw int64 data columns.  Fixed summation order: the same inputs give the same
+    bits.  Returns acc."""
+    _need_cuda(pred, pos_num, neg_num, acc)
+    if pred.dtype != torch.float32 or pred.dim() != 2 or pred.stride(1) != 1:
+        raise TypeError("impression_metrics: pred must be float32 [Bn, C] with contiguous rows")
+    pos_num, neg_num = _i64c(pos_num.reshape(-1), "pos_num"), _i64c(neg_num.reshape(-1), "neg_num")
+    Bn, Cn = pred.shape
+    ks = [int(k) for k in topk]
+    nk = len(ks)
+    if not 1 <= nk <= _lib.IMPRESSION_MAX_TOPK or min(ks) < 1:
+        raise ValueError(f"impression_metrics: 1 to {_lib.IMPRESSION_MAX_TOPK} cut-offs >= 1 expected, got {ks}")
+    if not 0 <= int(mp) <= Cn or pos_num.numel() != Bn or neg_num.numel() != Bn:
+        raise ValueError("impression_metrics: mp within the row, one pos_num / neg_num per row")
+    if acc.dtype != torch.float64 or not acc.is_contiguous() or acc.numel() != 3 * nk:
+        raise ValueError("impression_metrics: acc must be a contiguous float64 [3 * len(topk)] tensor")
+    if Bn == 0:
+        return acc
+    L = _lib.load()
+    nb = int(L.b2r_impression_metrics_workspace_bytes(Bn, Cn, nk))
+    key = acc.device.index if acc.device.index is not None else torch.cuda.current_device()
+    ws = _imp_ws.get(key)
+    if ws is None or ws.numel() < nb:
+        ws = _imp_ws[key] = torch.zeros(nb, dtype=torch.uint8, device=acc.device)   # the counter starts at zero
+    kk = (C.c_int * nk)(*ks)
+    _lib.check(L.b2r_impression_metrics(_p(pred), pred.stride(0), Bn, Cn, int(mp), _p(pos_num), _p(neg_num), kk, nk,
+                                        _p(acc), _p(ws), ws.numel(), _stream()), "b2r_impression_metrics")
+    return acc
+
+
 def adam_exact_advance(W: torch.Tensor, m: torch.Tensor, v: torch.Tensor, last: torch.Tensor, upto: int, opt,
                        rows: Optional[torch.Tensor] = None, stamp: int = 0, state_ld: int = 0) -> None:
     """Groundwork for the exact dense-Adam mode (b2r_adam_exact_advance): bring the listed unique rows (all rows when

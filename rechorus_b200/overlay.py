@@ -9,7 +9,8 @@ that graft this package's kernel mixins onto the reference's own ``GeneralModel`
 reference's Dataset, reader, runner, argument plumbing and checkpoint code are the ones that run), replaces
 ``models.general.BPRMF.BPRMF`` etc. with them, and ``runpy``s ``main.py``.  With ``--fused_step 1``,
 ``--device_metrics 1``, ``--device_batches N`` or ``--device_rec 1`` on the command line it also registers ``helpers.B200Runner`` (a subclass of the reference's own
-BaseRunner) through the same by-name discovery.  Needs a CUDA device for the first forward call; there is no CPU
+BaseRunner) through the same by-name discovery, and ``helpers.B200ImpressionRunner`` (a subclass of its ImpressionRunner)
+for the impression models.  Needs a CUDA device for the first forward call; there is no CPU
 fallback.  ``--ref`` defaults to the unmodified copy build() stages in oracle/_ref/src (oracle/stage_reference.py).
 """
 from __future__ import annotations
@@ -85,6 +86,37 @@ def _make_runner_module(ref_runner_cls):
 
     mod = types.ModuleType("helpers.B200Runner")
     mod.B200Runner = B200Runner
+    return mod
+
+
+def _make_impression_runner_module(ref_runner_cls):
+    """``helpers.B200ImpressionRunner``: the reference's own ImpressionRunner (fit / predict / print_res / logging
+    untouched) with evaluate() re-pointed at the device when the unchanged ``main.py`` parsed ``--device_metrics 1``
+    (runner.impression_device_route says when; runner.evaluate_impression_on_device does it).  Every other call is the
+    reference's evaluate()."""
+    import types
+
+    from . import runner as ours
+
+    class B200ImpressionRunner(ref_runner_cls):
+        @staticmethod
+        def parse_runner_args(parser):
+            parser = ref_runner_cls.parse_runner_args(parser)
+            parser.add_argument("--device_metrics", type=int, default=0,
+                                help="1: collate the evaluation batches and compute NDCG / MAP / HR on the GPU")
+            return parser
+
+        def __init__(self, args):
+            super().__init__(args)
+            self.device_metrics = getattr(args, "device_metrics", 0)
+
+        def evaluate(self, data, topks, metrics, check_sort_idx=0, all=0):
+            if ours.impression_device_route(self, data, check_sort_idx, all):
+                return ours.evaluate_impression_on_device(self, data, topks)
+            return super().evaluate(data, topks, metrics, check_sort_idx, all)
+
+    mod = types.ModuleType("helpers.B200ImpressionRunner")
+    mod.B200ImpressionRunner = B200ImpressionRunner
     return mod
 
 
@@ -173,7 +205,8 @@ def install(ref_src: str = DEFAULT_REF, b200_runner: bool = False):
     class _ImpLoss:
         def loss(self, out_dict, target=None):
             from . import ops
-            return ops.listwise_loss(out_dict["prediction"], target, self.loss_n, self.train_max_pos_item)
+            # ImpressionRunner.fit builds its labels with .int() (ImpressionRunner.py:187-190); the kernel reads int64
+            return ops.listwise_loss(out_dict["prediction"], target.long(), self.loss_n, self.train_max_pos_item)
 
     class BPRMFImpression(_ImpLoss, plugin.BPRMFKernels, RI.ImpressionModel):
         reader, runner = "ImpressionReader", "ImpressionRunner"
@@ -209,13 +242,16 @@ def install(ref_src: str = DEFAULT_REF, b200_runner: bool = False):
         # the model classes choose it (main.py:166: eval('{0}.{0}'.format(model_name.runner)))
         import helpers
         import helpers.BaseRunner as ref_runner
-        mod = _make_runner_module(ref_runner.BaseRunner)
-        sys.modules["helpers.B200Runner"] = mod
-        helpers.B200Runner = mod
-        if "B200Runner" not in helpers.__all__:
-            helpers.__all__.append("B200Runner")
-        for cls in (BPRMF, NeuMF, SASRec):
-            cls.runner = "B200Runner"
+        import helpers.ImpressionRunner as ref_imp_runner
+        for name, mod, classes in (("B200Runner", _make_runner_module(ref_runner.BaseRunner), (BPRMF, NeuMF, SASRec)),
+                                   ("B200ImpressionRunner", _make_impression_runner_module(ref_imp_runner.ImpressionRunner),
+                                    (BPRMFImpression, SASRecImpression))):
+            sys.modules["helpers." + name] = mod
+            setattr(helpers, name, mod)
+            if name not in helpers.__all__:
+                helpers.__all__.append(name)
+            for cls in classes:
+                cls.runner = name
     return {"BPRMF": BPRMF, "NeuMF": NeuMF, "SASRec": SASRec, "BPRMFImpression": BPRMFImpression,
             "SASRecImpression": SASRecImpression}
 

@@ -136,6 +136,114 @@ def device_eval_batches(dataset, B: int):
         yield feed, clicked
 
 
+def _impression_state(dataset, B: int) -> dict:
+    """The device inputs of one impression evaluation phase, uploaded when the device route first evaluates it and cached
+    on the dataset (as _eval_state does): users, the raw pos_num / neg_num columns, CSRs of the positive and negative
+    lists cut to test_max_pos_item / test_max_neg_item (ops.list_csr), the positive-history CSR (sequential models), and
+    batch buffers for eval_batch_size B."""
+    model = dataset.model
+    data, corpus, dev = dataset.data, dataset.corpus, model.device
+    mp, mn = int(model.test_max_pos_item), int(model.test_max_neg_item)
+    st = dataset.__dict__.get("_b2r_imp")
+    if st is None or st["mp"] != mp or st["mn"] != mn or st["pos_src"] is not data["pos_items"] \
+            or st["neg_src"] is not data["neg_items"]:
+        def up(a):
+            return torch.as_tensor(np.asarray(a, dtype=np.int64)).to(dev)
+        pos_ptr, pos_items = ops.list_csr(data["pos_items"], mp)
+        neg_ptr, neg_items = ops.list_csr(data["neg_items"], mn)
+        st = {"mp": mp, "mn": mn, "pos_src": data["pos_items"], "neg_src": data["neg_items"], "B": None,
+              "users": up(data["user_id"]), "pos_num": up(data["pos_num"]), "neg_num": up(data["neg_num"]),
+              "pos_ptr": up(pos_ptr), "pos_items": up(pos_items), "neg_ptr": up(neg_ptr), "neg_items": up(neg_items)}
+        if hasattr(model, "history_max"):
+            # ImpressionSeqModel.Dataset slices user_his[u]['pos'][:position] (BaseImpressionModel.py:206-214)
+            his = {u: h["pos"] for u, h in corpus.user_his.items()}
+            st["his"] = ops.DeviceHistory(his, corpus.n_users, data["user_id"], data["position"], model.history_max, dev)
+            pos = np.asarray(data["position"], dtype=np.int64)
+            H = int(model.history_max)
+            st["lens"] = np.minimum(pos, H) if H > 0 else pos
+        dataset.__dict__["_b2r_imp"] = st
+    if st["B"] != B:
+        bufs = {"user_id": torch.empty(B, dtype=torch.int64, device=dev),
+                "item_id": torch.empty((B, mp + mn), dtype=torch.int64, device=dev)}
+        if "his" in st:
+            bufs["history_items"] = torch.empty(B * st["his"].width, dtype=torch.int64, device=dev)
+            bufs["lengths"] = torch.empty(B, dtype=torch.int64, device=dev)
+            st["widths"] = eval_history_widths(st["lens"], B)
+        st["bufs"], st["B"] = bufs, B
+    return st
+
+
+def device_impression_batches(dataset, B: int):
+    """Yields (first row, feed dict) for the batches of B rows of an impression evaluation phase (an ImpressionModel /
+    ImpressionSeqModel Dataset, not under test_all), in dataset order, built on the device with the values
+    collate_batch gives (models/BaseImpressionModel.py:152-184, :200-240): ``user_id``, ``item_id`` = [pos_items[:mp] |
+    0-pad | neg_items[:mn] | 0-pad] (b2r_collate_impression), and for sequential models ``history_items`` / ``lengths``,
+    user_his[u]['pos'][:position] cut to history_max and right-padded to the batch's longest (b2r_collate_history).
+    ``pos_num`` / ``neg_num``, ``neg_history_items``, ``neg_lengths`` and the time columns are not produced: no
+    kernel-backed forward reads them.  Item ids are copied exactly (the reference's float32 padding step rounds ids
+    above 2^24).  Consecutive batches share the buffers: a batch must be consumed (its work enqueued on the current
+    stream) before the next one is requested."""
+    model = dataset.model
+    B = int(B)
+    st = _impression_state(dataset, B)
+    bufs, his, users = st["bufs"], st.get("his"), st["users"]
+    N = users.numel()
+    for bi, start in enumerate(range(0, N, B)):
+        Bn = min(B, N - start)
+        ops.collate_impression(users, st["pos_ptr"], st["pos_items"], st["neg_ptr"], st["neg_items"],
+                               dataset.corpus.n_users, start, Bn, st["mp"], st["mn"], bufs["user_id"], bufs["item_id"])
+        feed = {"batch_size": Bn, "phase": dataset.phase, "user_id": bufs["user_id"][:Bn],
+                "item_id": bufs["item_id"][:Bn]}
+        if his is not None:
+            hb = history_view(bufs["history_items"], Bn, st["widths"][bi])
+            his.collate(users, None, start, Bn, hb, bufs["lengths"])
+            feed["history_items"], feed["lengths"] = hb, bufs["lengths"][:Bn]
+        yield start, feed
+
+
+def impression_device_route(runner, dataset, check_sort_idx=0, all=0) -> bool:
+    """Whether ImpressionRunner.evaluate (helpers/ImpressionRunner.py:135-171) can run as
+    evaluate_impression_on_device: --device_metrics 1, no test_all (the reference computes no metrics there),
+    neither check_sort_idx nor all (its logging and per-row returns), mn <= mp (beyond that the reference's 2 * mp wide
+    label matrix raises IndexError), a pos_num column (without one :171 passes check_sort_idx as pos_num), at least one
+    row, and a kernel-backed model.  Everything else keeps the reference's route."""
+    model = dataset.model
+    data = dataset.data
+    return bool(getattr(runner, "device_metrics", 0)) and not getattr(model, "test_all", 0) \
+        and check_sort_idx == 0 and all == 0 \
+        and int(model.test_max_neg_item) <= int(model.test_max_pos_item) \
+        and "pos_num" in data and len(data["neg_num"]) > 0 and hasattr(model, "eval_ranks")
+
+
+def evaluate_impression_on_device(runner, dataset, topks: list) -> Dict[str, float]:
+    """ImpressionRunner.evaluate + evaluate_method (helpers/ImpressionRunner.py:135-171, :74-133, non-test_all branch)
+    with neither the inputs nor the predictions on the host: batches from device_impression_batches, the model's
+    predictions of each batch ranked and scored by b2r_impression_metrics into one float64 accumulator, and the
+    3 * len(topks) sums read once.  Returns NDCG@k for every k, then MAP@k, then HR@k (evaluate_method ignores
+    --metric), each the float64 mean over the rows, as the reference does; the summation order differs from NumPy's,
+    so values agree to about 1e-12, not bit for bit (DESIGN.md §6)."""
+    model = dataset.model
+    model.eval()
+    ks = [int(k) for k in topks]
+    # the host route's DataLoader iterator draws one int64 seed from the global CPU generator: draw it here too
+    torch.empty((), dtype=torch.int64).random_()
+    st = _impression_state(dataset, int(runner.eval_batch_size))
+    acc = torch.zeros(3 * len(ks), dtype=torch.float64, device=model.device)
+    fn = model.inference if hasattr(model, "inference") else model
+    for start, feed in device_impression_batches(dataset, runner.eval_batch_size):
+        Bn = feed["batch_size"]
+        pred = fn(feed)["prediction"].contiguous()
+        ops.impression_metrics(pred, st["pos_num"][start:start + Bn], st["neg_num"][start:start + Bn], st["mp"], ks, acc)
+    _poll_ids(model)
+    sums = acc.cpu().numpy()
+    N = st["users"].numel()
+    out = {}
+    for m, name in enumerate(("NDCG", "MAP", "HR")):
+        for i, k in enumerate(ks):
+            out[f"{name}@{k}"] = np.float64(sums[m * len(ks) + i] / N)
+    return out
+
+
 class BaseRunner:
     @staticmethod
     def parse_runner_args(parser):
