@@ -492,8 +492,9 @@ B2R_API int b2r_topk_all_items(const float* Q, int ldq, const float* I, int64_t 
                                void* workspace, size_t workspace_bytes, b2r_stream_t stream);
 
 /* ------------------------------------------------------------------------------------------------
- * Impression evaluation (row f4): ImpressionRunner.evaluate (helpers/ImpressionRunner.py:135-171) for the
- * non-test_all branch on the device, batch by batch, without feed dicts or a host copy of the predictions.
+ * Impression evaluation and training batches (row f4): ImpressionRunner.evaluate (helpers/ImpressionRunner.py:135-171)
+ * for the non-test_all branch on the device, batch by batch, without feed dicts or a host copy of the predictions; and
+ * the batches and labels of ImpressionRunner.fit (:173-197) in the DataLoader's shuffled order.
  *
  * b2r_collate_impression: rows [start, start + Bn) of an evaluation phase as ImpressionModel.Dataset builds them
  *                     (models/BaseImpressionModel.py:152-184): out_uid int64 [Bn] = users[start + t], out_iid int64
@@ -501,6 +502,13 @@ B2R_API int b2r_topk_all_items(const float* Q, int ldq, const float* I, int64_t 
  *                     phase's rows: row r's positives at pos_items[pos_ptr[r] .. pos_ptr[r + 1]), its negatives at
  *                     neg_items[neg_ptr[r] .. neg_ptr[r + 1]); only the first mp / mn entries are read.  A user outside
  *                     [0, n_users) is clamped to 0 and counted in err_flag.
+ * b2r_collate_impression_train: the same for one training batch whose rows are perm[start + t] (perm int64, indices of
+ *                     the phase's rows; NULL: start + t), plus the labels ImpressionRunner.fit builds (:186-189) in out_labels int64
+ *                     [Bn, mp + mn].  With P = min(pos_num[row], mp) and Q = min(neg_num[row], mn) -- the raw data
+ *                     columns clipped as _get_feed_dict clips them (models/BaseImpressionModel.py:178-179):
+ *                       - column c < mp: 1 if c < P, else -1;
+ *                       - column c >= mp: 0 if c - mp < Q, else -1.
+ *                     b2r_collate_impression runs the same kernel without a permutation or labels.
  * b2r_impression_metrics: adds the per-row NDCG@k, MAP@k and HR@k of one batch's predictions pred [Bn, C] (row stride ld,
  *                     C = mp + mn) into acc float64 [3 * nk]: acc[i] += sum of NDCG@topk[i], acc[nk + i] += sum of MAP@..,
  *                     acc[2 nk + i] += sum of HR@..; the caller divides by the row count.  pos_num / neg_num int64 [Bn]
@@ -528,6 +536,11 @@ B2R_API int b2r_collate_impression(const int64_t* users, const int64_t* pos_ptr,
                                    const int64_t* neg_ptr, const int64_t* neg_items, int64_t n_users, int64_t start,
                                    int Bn, int mp, int mn, int64_t* out_uid, int64_t* out_iid, int32_t* err_flag,
                                    b2r_stream_t stream);
+B2R_API int b2r_collate_impression_train(const int64_t* users, const int64_t* pos_ptr, const int64_t* pos_items,
+                                         const int64_t* neg_ptr, const int64_t* neg_items, const int64_t* pos_num,
+                                         const int64_t* neg_num, const int64_t* perm, int64_t n_users, int64_t start,
+                                         int Bn, int mp, int mn, int64_t* out_uid, int64_t* out_iid, int64_t* out_labels,
+                                         int32_t* err_flag, b2r_stream_t stream);
 B2R_API size_t b2r_impression_metrics_workspace_bytes(int Bn, int C, int nk);
 B2R_API int b2r_impression_metrics(const float* pred, int64_t ld, int Bn, int C, int mp, const int64_t* pos_num,
                                    const int64_t* neg_num, const int* topk, int nk, double* acc, void* workspace,

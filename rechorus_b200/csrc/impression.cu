@@ -3,8 +3,10 @@
 // ImpressionRunner.evaluate + evaluate_method (helpers/ImpressionRunner.py:135-171, :74-133), so neither one feed dict
 // per impression nor the [N, mp + mn] prediction matrix has to exist on the host.
 //
-//   k_collate_impression   item_id[t] = [pos[:mp] | 0-pad to mp | neg[:mn] | 0-pad to mn] of phase row start + t, from a
-//                          CSR of the (truncated) positive and negative lists; user_id[t] = users[start + t]
+//   k_collate_impression   item_id[t] = [pos[:mp] | 0-pad to mp | neg[:mn] | 0-pad to mn] of phase row
+//                          perm[start + t] (start + t without a permutation), from a CSR of the (truncated) positive and
+//                          negative lists; user_id[t] = users[row]; for a training batch also ImpressionRunner.fit's
+//                          labels (helpers/ImpressionRunner.py:186-189) from the row's pos_num / neg_num
 //   k_impression_metrics   one warp per row: the row's float64 sort keys staged in shared memory, every valid positive
 //                          ranked by counting the columns the reference's stable argsort puts before it, NDCG / MAP / HR
 //                          for every cut-off from those ranks, per-CTA sums, and a last-CTA pass that adds the CTA sums
@@ -41,20 +43,23 @@ static inline int imp_warps(int C) {
     return n < 1 ? 1 : (n > kImpMaxWarps ? kImpMaxWarps : n);
 }
 
-// One phase batch: rows [start, start + Bn) of the phase.  Row `row` has the positive list
+// One phase batch: rows perm[start + t] (perm NULL: start + t) for t < Bn.  Row `row` has the positive list
 // pos_items[pos_ptr[row] .. pos_ptr[row + 1]) and the negative list neg_items[neg_ptr[row] .. neg_ptr[row + 1]);
 // only their first mp / mn entries are read, as the slices target_item[:pos_len] / neg_items[:neg_len] of
-// _get_feed_dict take them, and the rest of each half is 0 as collate_batch pads it.
+// _get_feed_dict take them, and the rest of each half is 0 as collate_batch pads it.  With out_lab (a training batch),
+// label[t, c] = c < min(pos_num[row], mp) ? 1 : -1 for c < mp and c - mp < min(neg_num[row], mn) ? 0 : -1 after it.
 __global__ void __launch_bounds__(256)
 k_collate_impression(const int64_t* __restrict__ users, const int64_t* __restrict__ pos_ptr,
                      const int64_t* __restrict__ pos_items, const int64_t* __restrict__ neg_ptr,
-                     const int64_t* __restrict__ neg_items, int64_t n_users, int64_t start, int Bn, int mp, int mn,
-                     int64_t* __restrict__ out_uid, int64_t* __restrict__ out_iid, int32_t* __restrict__ err_flag) {
+                     const int64_t* __restrict__ neg_items, const int64_t* __restrict__ pos_num,
+                     const int64_t* __restrict__ neg_num, const int64_t* __restrict__ perm, int64_t n_users,
+                     int64_t start, int Bn, int mp, int mn, int64_t* __restrict__ out_uid, int64_t* __restrict__ out_iid,
+                     int64_t* __restrict__ out_lab, int32_t* __restrict__ err_flag) {
     const int C = mp + mn;
     const int64_t total = (int64_t)Bn * C;
     for (int64_t idx = (int64_t)blockIdx.x * 256 + threadIdx.x; idx < total; idx += (int64_t)gridDim.x * 256) {
         const int t = (int)(idx / C), c = (int)(idx - (int64_t)t * C);
-        const int64_t row = start + t;
+        const int64_t row = perm ? perm[start + t] : start + t;
         if (c == 0) {
             int64_t u = users[row];
             if (u < 0 || u >= n_users) {
@@ -63,15 +68,18 @@ k_collate_impression(const int64_t* __restrict__ users, const int64_t* __restric
             }
             out_uid[t] = u;
         }
-        int64_t v = 0;
+        int64_t v = 0, lab = -1;
         if (c < mp) {
             const int64_t b = pos_ptr[row];
             if (c < pos_ptr[row + 1] - b) v = pos_items[b + c];
+            if (out_lab && c < min(pos_num[row], (int64_t)mp)) lab = 1;
         } else {
             const int64_t b = neg_ptr[row];
             if (c - mp < neg_ptr[row + 1] - b) v = neg_items[b + (c - mp)];
+            if (out_lab && c - mp < min(neg_num[row], (int64_t)mn)) lab = 0;
         }
         out_iid[idx] = v;
+        if (out_lab) out_lab[idx] = lab;
     }
 }
 
@@ -204,24 +212,44 @@ k_impression_metrics(const float* __restrict__ pred, int64_t ld, int Bn, int C, 
 
 using namespace b2r;
 
-extern "C" int b2r_collate_impression(const int64_t* users, const int64_t* pos_ptr, const int64_t* pos_items,
-                                      const int64_t* neg_ptr, const int64_t* neg_items, int64_t n_users, int64_t start,
-                                      int Bn, int mp, int mn, int64_t* out_uid, int64_t* out_iid, int32_t* err_flag,
-                                      b2r_stream_t stream) {
+static int collate_impression(const char* name, const int64_t* users, const int64_t* pos_ptr, const int64_t* pos_items,
+                              const int64_t* neg_ptr, const int64_t* neg_items, const int64_t* pos_num,
+                              const int64_t* neg_num, const int64_t* perm, int64_t n_users, int64_t start, int Bn, int mp,
+                              int mn, int64_t* out_uid, int64_t* out_iid, int64_t* out_lab, int32_t* err_flag,
+                              b2r_stream_t stream) {
     B2R_REQUIRE(users && pos_ptr && pos_items && neg_ptr && neg_items && out_uid && out_iid, B2R_E_BADARG,
-                "b2r_collate_impression: null pointer");
+                "%s: null pointer", name);
     B2R_REQUIRE(Bn >= 0 && start >= 0 && mp >= 0 && mn >= 0 && mp + mn >= 1 && n_users >= 1, B2R_E_BADARG,
-                "b2r_collate_impression: Bn=%d start=%lld mp=%d mn=%d n_users=%lld", Bn, (long long)start, mp, mn,
+                "%s: Bn=%d start=%lld mp=%d mn=%d n_users=%lld", name, Bn, (long long)start, mp, mn,
                 (long long)n_users);
     if (Bn == 0) return 0;
     const int64_t total = (int64_t)Bn * (mp + mn);
     int64_t grid = (total + 255) / 256;
     const int64_t cap = (int64_t)sm_count() * 8;
     if (grid > cap) grid = cap;
-    k_collate_impression<<<(int)grid, 256, 0, as_stream(stream)>>>(users, pos_ptr, pos_items, neg_ptr, neg_items, n_users,
-                                                                   start, Bn, mp, mn, out_uid, out_iid, err_flag);
+    k_collate_impression<<<(int)grid, 256, 0, as_stream(stream)>>>(users, pos_ptr, pos_items, neg_ptr, neg_items, pos_num,
+                                                                   neg_num, perm, n_users, start, Bn, mp, mn, out_uid,
+                                                                   out_iid, out_lab, err_flag);
     B2R_LAUNCH_OK("k_collate_impression");
     return 0;
+}
+
+extern "C" int b2r_collate_impression(const int64_t* users, const int64_t* pos_ptr, const int64_t* pos_items,
+                                      const int64_t* neg_ptr, const int64_t* neg_items, int64_t n_users, int64_t start,
+                                      int Bn, int mp, int mn, int64_t* out_uid, int64_t* out_iid, int32_t* err_flag,
+                                      b2r_stream_t stream) {
+    return collate_impression("b2r_collate_impression", users, pos_ptr, pos_items, neg_ptr, neg_items, nullptr, nullptr,
+                              nullptr, n_users, start, Bn, mp, mn, out_uid, out_iid, nullptr, err_flag, stream);
+}
+
+extern "C" int b2r_collate_impression_train(const int64_t* users, const int64_t* pos_ptr, const int64_t* pos_items,
+                                            const int64_t* neg_ptr, const int64_t* neg_items, const int64_t* pos_num,
+                                            const int64_t* neg_num, const int64_t* perm, int64_t n_users, int64_t start,
+                                            int Bn, int mp, int mn, int64_t* out_uid, int64_t* out_iid,
+                                            int64_t* out_labels, int32_t* err_flag, b2r_stream_t stream) {
+    B2R_REQUIRE(pos_num && neg_num && out_labels, B2R_E_BADARG, "b2r_collate_impression_train: null pointer");
+    return collate_impression("b2r_collate_impression_train", users, pos_ptr, pos_items, neg_ptr, neg_items, pos_num,
+                              neg_num, perm, n_users, start, Bn, mp, mn, out_uid, out_iid, out_labels, err_flag, stream);
 }
 
 extern "C" size_t b2r_impression_metrics_workspace_bytes(int Bn, int C, int nk) {

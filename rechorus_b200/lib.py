@@ -167,6 +167,9 @@ SIGNATURES = {
                                      C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p]),
     "b2r_collate_impression": (C.c_int, [C.c_void_p] * 5 + [C.c_int64, C.c_int64, C.c_int, C.c_int, C.c_int,
                                                             C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "b2r_collate_impression_train": (C.c_int, [C.c_void_p] * 8 + [C.c_int64, C.c_int64, C.c_int, C.c_int, C.c_int,
+                                                                  C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
+                                                                  C.c_void_p]),
     "b2r_impression_metrics_workspace_bytes": (C.c_size_t, [C.c_int, C.c_int, C.c_int]),
     "b2r_impression_metrics": (C.c_int, [C.c_void_p, C.c_int64, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p,
                                          C.POINTER(C.c_int), C.c_int, C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p]),

@@ -581,6 +581,34 @@ def collate_impression(users: torch.Tensor, pos_ptr: torch.Tensor, pos_items: to
                "b2r_collate_impression")
 
 
+def collate_impression_train(users: torch.Tensor, pos_ptr: torch.Tensor, pos_items: torch.Tensor, neg_ptr: torch.Tensor,
+                             neg_items: torch.Tensor, pos_num: torch.Tensor, neg_num: torch.Tensor,
+                             perm: Optional[torch.Tensor], n_users: int, start: int, Bn: int, mp: int, mn: int, out_uid: torch.Tensor,
+                             out_iid: torch.Tensor, out_labels: torch.Tensor) -> None:
+    """b2r_collate_impression_train: one training batch of ImpressionRunner.fit (helpers/ImpressionRunner.py:181-190), the
+    rows perm[start:start + Bn] of the training set (perm None: rows start .. start + Bn - 1): ``user_id`` and ``item_id`` as collate_impression builds them, and
+    out_labels[t, c] = 1 / -1 for c < mp (c < min(pos_num, mp)) and 0 / -1 after it (c - mp < min(neg_num, mn)).
+    pos_num / neg_num are the raw int64 data columns of the whole set.  A user outside [0, n_users) makes check_ids
+    raise IndexError."""
+    tensors = (users, pos_ptr, pos_items, neg_ptr, neg_items, pos_num, neg_num, perm, out_uid, out_iid, out_labels)
+    _need_cuda(*tensors)
+    for t in tensors:
+        if t is not None and (t.dtype != torch.int64 or not t.is_contiguous()):
+            raise TypeError("collate_impression_train: contiguous int64 tensors expected")
+    N = users.numel()
+    if pos_ptr.numel() != N + 1 or neg_ptr.numel() != N + 1 or pos_num.numel() != N or neg_num.numel() != N:
+        raise ValueError("collate_impression_train: CSRs and pos_num / neg_num that do not cover the set's rows")
+    if (perm is not None and perm.numel() != N) or not 0 <= start <= start + Bn <= N:
+        raise ValueError("collate_impression_train: perm must order the set's rows, and the batch must lie within it")
+    if (out_iid.dim() != 2 or out_iid.shape[1] != mp + mn or out_iid.shape[0] < Bn or out_uid.numel() < Bn
+            or out_labels.shape != out_iid.shape):
+        raise ValueError("collate_impression_train: output buffers do not fit the batch")
+    _lib.check(_lib.load().b2r_collate_impression_train(
+        _p(users), _p(pos_ptr), _p(pos_items), _p(neg_ptr), _p(neg_items), _p(pos_num), _p(neg_num), _p(perm),
+        int(n_users), int(start), int(Bn), int(mp), int(mn), _p(out_uid), _p(out_iid), _p(out_labels),
+        _p(err_flag(users.device)), _stream()), "b2r_collate_impression_train")
+
+
 _imp_ws = {}
 
 

@@ -90,10 +90,13 @@ def _make_runner_module(ref_runner_cls):
 
 
 def _make_impression_runner_module(ref_runner_cls):
-    """``helpers.B200ImpressionRunner``: the reference's own ImpressionRunner (fit / predict / print_res / logging
-    untouched) with evaluate() re-pointed at the device when the unchanged ``main.py`` parsed ``--device_metrics 1``
-    (runner.impression_device_route says when; runner.evaluate_impression_on_device does it).  Every other call is the
-    reference's evaluate()."""
+    """``helpers.B200ImpressionRunner``: the reference's own ImpressionRunner (predict / print_res / logging untouched)
+    with two seams re-pointed at the device by flags the unchanged ``main.py`` parses for us:
+      --device_metrics 1  evaluate() collates the batches and computes NDCG / MAP / HR on the GPU
+                          (runner.impression_device_route says when; runner.evaluate_impression_on_device does it);
+      --device_batches N  fit() builds every training batch and its labels on the GPU in the reference DataLoader's own
+                          order (runner.impression_train_device_route says when; runner.fit_impression_on_device does it).
+    Every other call is the reference's."""
     import types
 
     from . import runner as ours
@@ -104,11 +107,20 @@ def _make_impression_runner_module(ref_runner_cls):
             parser = ref_runner_cls.parse_runner_args(parser)
             parser.add_argument("--device_metrics", type=int, default=0,
                                 help="1: collate the evaluation batches and compute NDCG / MAP / HR on the GPU")
+            parser.add_argument("--device_batches", type=int, default=0,
+                                help="non-zero: collate every training batch and its labels on the GPU, in the order the "
+                                     "host route shuffles them; the value is not a seed here (nothing is sampled)")
             return parser
 
         def __init__(self, args):
             super().__init__(args)
             self.device_metrics = getattr(args, "device_metrics", 0)
+            self.device_batches = getattr(args, "device_batches", 0)
+
+        def fit(self, data, epoch=-1):
+            if ours.impression_train_device_route(self, data):
+                return ours.fit_impression_on_device(self, data, epoch)
+            return super().fit(data, epoch)
 
         def evaluate(self, data, topks, metrics, check_sort_idx=0, all=0):
             if ours.impression_device_route(self, data, check_sort_idx, all):

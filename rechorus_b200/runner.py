@@ -136,14 +136,14 @@ def device_eval_batches(dataset, B: int):
         yield feed, clicked
 
 
-def _impression_state(dataset, B: int) -> dict:
-    """The device inputs of one impression evaluation phase, uploaded when the device route first evaluates it and cached
-    on the dataset (as _eval_state does): users, the raw pos_num / neg_num columns, CSRs of the positive and negative
-    lists cut to test_max_pos_item / test_max_neg_item (ops.list_csr), the positive-history CSR (sequential models), and
-    batch buffers for eval_batch_size B."""
+def _impression_state(dataset, B: int, mp: int, mn: int) -> dict:
+    """The device inputs of one impression phase, uploaded when a device route first uses it and cached on the dataset
+    (as _eval_state does): users, the raw pos_num / neg_num columns, CSRs of the positive and negative lists cut to mp /
+    mn (ops.list_csr; test_max_* for evaluation, train_max_* for training), the positive-history CSR (sequential models),
+    and batch buffers for batches of B rows."""
     model = dataset.model
     data, corpus, dev = dataset.data, dataset.corpus, model.device
-    mp, mn = int(model.test_max_pos_item), int(model.test_max_neg_item)
+    mp, mn = int(mp), int(mn)
     st = dataset.__dict__.get("_b2r_imp")
     if st is None or st["mp"] != mp or st["mn"] != mn or st["pos_src"] is not data["pos_items"] \
             or st["neg_src"] is not data["neg_items"]:
@@ -185,7 +185,7 @@ def device_impression_batches(dataset, B: int):
     stream) before the next one is requested."""
     model = dataset.model
     B = int(B)
-    st = _impression_state(dataset, B)
+    st = _impression_state(dataset, B, model.test_max_pos_item, model.test_max_neg_item)
     bufs, his, users = st["bufs"], st.get("his"), st["users"]
     N = users.numel()
     for bi, start in enumerate(range(0, N, B)):
@@ -227,7 +227,7 @@ def evaluate_impression_on_device(runner, dataset, topks: list) -> Dict[str, flo
     ks = [int(k) for k in topks]
     # the host route's DataLoader iterator draws one int64 seed from the global CPU generator: draw it here too
     torch.empty((), dtype=torch.int64).random_()
-    st = _impression_state(dataset, int(runner.eval_batch_size))
+    st = _impression_state(dataset, int(runner.eval_batch_size), model.test_max_pos_item, model.test_max_neg_item)
     acc = torch.zeros(3 * len(ks), dtype=torch.float64, device=model.device)
     fn = model.inference if hasattr(model, "inference") else model
     for start, feed in device_impression_batches(dataset, runner.eval_batch_size):
@@ -241,6 +241,79 @@ def evaluate_impression_on_device(runner, dataset, topks: list) -> Dict[str, flo
     for m, name in enumerate(("NDCG", "MAP", "HR")):
         for i, k in enumerate(ks):
             out[f"{name}@{k}"] = np.float64(sums[m * len(ks) + i] / N)
+    return out
+
+
+def reference_shuffle(N: int) -> torch.Tensor:
+    """The row order of one epoch of ``DataLoader(dataset, shuffle=True)`` without a generator, drawn from the global CPU
+    generator exactly as torch draws it (any num_workers): ``_BaseDataLoaderIter.__init__`` takes one int64 for its
+    ``_base_seed`` (torch/utils/data/dataloader.py), then ``RandomSampler.__iter__`` takes a second as the seed of a fresh
+    Generator and yields ``torch.randperm(N, generator=...)`` (torch/utils/data/sampler.py).  Returns that CPU int64 [N]
+    permutation and leaves the global generator where the DataLoader's epoch leaves it."""
+    torch.empty((), dtype=torch.int64).random_()
+    seed = int(torch.empty((), dtype=torch.int64).random_().item())
+    return torch.randperm(int(N), generator=torch.Generator().manual_seed(seed))
+
+
+def impression_train_device_route(runner, dataset) -> bool:
+    """Whether ImpressionRunner.fit (helpers/ImpressionRunner.py:173-197) can run as fit_impression_on_device:
+    --device_batches set, a kernel-backed model, pos_num and neg_num columns (the labels are built from them) and at least
+    one row.  Everything else keeps the reference's route."""
+    data = dataset.data
+    return bool(getattr(runner, "device_batches", 0)) and hasattr(dataset.model, "eval_ranks") \
+        and "pos_num" in data and "neg_num" in data and len(data["neg_num"]) > 0
+
+
+def fit_impression_on_device(runner, dataset, epoch=-1) -> float:
+    """ImpressionRunner.fit (helpers/ImpressionRunner.py:173-197) step for step, with the batches built on the device:
+    the epoch's row order is the reference DataLoader's own (reference_shuffle, uploaded once), and per batch one
+    b2r_collate_impression_train launch writes ``user_id``, ``item_id`` and the labels, and for sequential models
+    b2r_collate_history the histories, right-padded to the batch's longest as collate_batch pads them.  The forward, the
+    loss on those labels, backward and optimizer.step are the reference's calls, so the epoch's losses, the parameters and
+    the CPU RNG state after it equal the host route's.  Each step's loss and a non-finite flag (loss or any prediction)
+    stay on the device and are read once, at the end of the epoch; every flagged step logs the reference's message (which
+    does not stop training).  Returns np.mean of the float32 losses, the reference's reduction.  One set of batch buffers
+    serves every step: each step's work is enqueued before the next collate overwrites them."""
+    model = dataset.model
+    if model.optimizer is None:
+        model.optimizer = runner._build_optimizer(model)
+    dataset.actions_before_epoch()
+    model.train()
+    dev = model.device
+    mp, mn, B = int(model.train_max_pos_item), int(model.train_max_neg_item), int(runner.batch_size)
+    st = _impression_state(dataset, B, mp, mn)
+    bufs, his, users = st["bufs"], st.get("his"), st["users"]
+    if "labels" not in bufs:
+        bufs["labels"] = torch.empty((B, mp + mn), dtype=torch.int64, device=dev)
+    N = users.numel()
+    order = reference_shuffle(N)
+    perm = order.to(dev)
+    widths = eval_history_widths(st["lens"][order.numpy()], B) if his is not None else None
+    n_steps = (N + B - 1) // B
+    losses = torch.empty(n_steps, dtype=torch.float32, device=dev)
+    bad = torch.empty(n_steps, dtype=torch.bool, device=dev)
+    for k, start in enumerate(range(0, N, B)):
+        Bn = min(B, N - start)
+        ops.collate_impression_train(users, st["pos_ptr"], st["pos_items"], st["neg_ptr"], st["neg_items"],
+                                     st["pos_num"], st["neg_num"], perm, dataset.corpus.n_users, start, Bn, mp, mn,
+                                     bufs["user_id"], bufs["item_id"], bufs["labels"])
+        feed = {"batch_size": Bn, "phase": dataset.phase, "user_id": bufs["user_id"][:Bn],
+                "item_id": bufs["item_id"][:Bn]}
+        if his is not None:
+            hb = history_view(bufs["history_items"], Bn, widths[k])
+            his.collate(users, perm, start, Bn, hb, bufs["lengths"])
+            feed["history_items"], feed["lengths"] = hb, bufs["lengths"][:Bn]
+        model.optimizer.zero_grad()
+        out = model(feed)
+        loss = model.loss(out, bufs["labels"][:Bn])
+        bad[k] = ~(torch.isfinite(loss.detach()).all() & torch.isfinite(out["prediction"].detach()).all())
+        loss.backward()
+        model.optimizer.step()
+        losses[k] = loss.detach().reshape(())
+    for _ in range(int(bad.sum())):
+        logging.info("Loss is Nan. Stop training at %d." % (epoch + 1))
+    out = np.mean(losses.cpu().numpy()).item()
+    _poll_ids(model)
     return out
 
 
