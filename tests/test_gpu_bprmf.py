@@ -353,46 +353,3 @@ def test_train_step_without_direct_plan_takes_autograd_route(monkeypatch):
         assert abs(losses[t] - float(lb)) <= 2e-6
     for (k, pa), (_, pb) in zip(ma.named_parameters(), mb.named_parameters()):
         assert (pa - pb).abs().max() <= 1e-6, k
-
-
-@pytest.mark.parametrize("n_rows,n,d,desc", [(1000, 5000, 64, "uniform"), (7, 2560, 64, "7 rows: long rows, one bucket each"),
-                                             (3, 9000, 64, "3 rows: oversize buckets (> 2048 pairs of one row)"),
-                                             (100000, 3000, 32, "sparse"), (50, 700, 128, "d=128"),
-                                             (40, 6000, 64, "hot rows + ignore id")])
-def test_direct_plan_matches_sorted_plan_and_is_reproducible(n_rows, n, d, desc):
-    """b2r_direct_plan_build + b2r_direct_plan_apply (shared-memory sort per bucket) vs the device-radix-sort plan:
-    same dense gradient, same bits on every run, also for hot rows, long rows (bitonic path), regions that spill and
-    buckets that overflow shared memory (chunk sort + merge)."""
-    from rechorus_b200 import lib as L, ops
-    g = torch.Generator().manual_seed(n_rows + n)
-    ids = torch.randint(0, n_rows, (n,), generator=g)
-    if "hot" in desc:
-        ids[::3] = 5
-        ids[1::7] = 0
-    ign = 0 if "ignore" in desc else -1
-    src = torch.randn(n, d, generator=g).cuda()
-    coef = torch.randn(n, generator=g).cuda()
-    source = ops.Source(src=src, n=n, coef=coef)
-    ref = torch.zeros(n_rows, d).cuda()
-    ops.IndexPlan(ids.cuda(), n_rows, ign, n if ign >= 0 else 0).add_to_dense(ref, [source])
-    outs = []
-    for _ in range(2):
-        out = torch.zeros(n_rows, d).cuda()
-        ops.DirectPlan(ids.cuda(), n_rows, ign, n if ign >= 0 else 0).add_to_dense(out, [source])
-        outs.append(out)
-    assert torch.equal(outs[0], outs[1])
-    want = torch.zeros(n_rows, d, dtype=torch.float64)
-    keep = ids != ign
-    want.index_add_(0, ids[keep], (coef.cpu().double().unsqueeze(1) * src.cpu().double())[keep])
-    scale = max(1.0, float(want.abs().max()))
-    assert (outs[0].cpu().double() - want).abs().max() <= 2e-6 * scale * max(1, n // n_rows) ** 0.5
-    assert (outs[0] - ref).abs().max() <= 1e-5 * scale
-    # fused optimizer through both paths: identical updates
-    W1 = torch.randn(n_rows, d, generator=g).cuda()
-    W2 = W1.clone()
-    opt = L.Optim(1, 0.01, 0.9, 0.999, 1e-3, 1e-4, 0.1, 0.001)
-    m1, v1, m2, v2 = [torch.zeros_like(W1) for _ in range(4)]
-    ops.IndexPlan(ids.cuda(), n_rows, ign, n if ign >= 0 else 0).apply_optimizer(W1, m1, v1, opt, [source])
-    ops.DirectPlan(ids.cuda(), n_rows, ign, n if ign >= 0 else 0).apply_optimizer(W2, m2, v2, opt, [source])
-    assert (W1 - W2).abs().max() <= 1e-5 and (m1 - m2).abs().max() <= 1e-5 * scale
-    ops.check_ids()
