@@ -1221,8 +1221,9 @@ def linear_bwd(dy: torch.Tensor, x: torch.Tensor, W: torch.Tensor, y_relu: Optio
         dx = torch.empty((M, K), dtype=torch.float32, device=dy.device)
         done = False
         Wd = W if drop is None else W * drop.scale
-        if M >= 4096 and N % 32 == 0 and N <= 128 and K % 16 == 0 and K <= 256 and lddy % 4 == 0:
-            # dX = (dY o mask) W = (dY o mask) (W^T)^T on the tensor-core kernel: the transposed weight (N*K floats) is a copy
+        if linear_fwd_uses_tc(M, K, N) and lddy % 4 == 0:
+            # dX = (dY o mask) W = (dY o mask) (W^T)^T on the tensor-core kernel, whose class (K output columns over a
+            # reduction of N) the library decides: the transposed weight (N*K floats) is a copy
             Wt = Wd.t().contiguous()
             rc = L.b2r_linear_tc(_p(dy), lddy, _p(y_relu), _p(Wt), None, _p(dx), K, M, K, N, 0, _stream())
             done = rc == 0
@@ -1273,7 +1274,7 @@ class _Linear(torch.autograd.Function):
             x2 = x2.contiguous()
         N, K = W.shape
         # a long batch dimension (M >= 4096) runs on the tensor cores (csrc/linear_tc.cu: wgmma, TF32 hi/lo split,
-        # 3 products, fp32-class accuracy checked in tests/test_gpu_tc.py); linear_bwd picks dX and dW the same way
+        # 3 products, fp32-class accuracy checked in tests/test_gpu_linear_tc.py); linear_bwd picks dX the same way
         tc = linear_fwd_uses_tc(x2.shape[0], N, K)
         if drop is not None:
             if not relu:
