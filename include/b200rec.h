@@ -492,6 +492,38 @@ B2R_API int b2r_topk_all_items(const float* Q, int ldq, const float* I, int64_t 
                                void* workspace, size_t workspace_bytes, b2r_stream_t stream);
 
 /* ------------------------------------------------------------------------------------------------
+ * The CSV of save_rec_results (main.py:117-132, TopK branch) written on the device: the text pandas' to_csv(sep=sep,
+ * index=False) gives for the DataFrame of user ids, Python lists of np.int64 item ids and Python lists of np.float32
+ * scores.  Format contract (pinned against NumPy 2.3 / pandas 3.0 by tests/test_rec_csv_cpu.py):
+ *   - the header "user_id<sep>rec_items<sep>rec_predictions\n" is the caller's; each of the N rows is
+ *     "<user><sep><items cell><sep><scores cell>\n";
+ *   - a cell is "[" + ", ".join(repr(e) for e in row) + "]", the user a plain decimal integer;
+ *   - QUOTE_MINIMAL: a field is wrapped in '"' exactly when it contains sep (sep ',' or ' ' quotes both cells of a row of
+ *     k >= 2, sep '1' quotes the user 10).  No text contains '"', '\r' or '\n', so nothing is escaped;
+ *   - element text in style B2R_REC_STYLE_NP (0, NumPy >= 2): "np.int64(<n>)" and "np.float32(<f>)"; in style
+ *     B2R_REC_STYLE_BARE (1, NumPy 1.x and legacy='1.25'): "<n>" and "<f>";
+ *   - <f> is NumPy's float32 scalar repr: the shortest decimal that reads back to the same float32 (the one closest to
+ *     the exact value when several have that length; Ryu, PAPERS.md), positional for 1e-4 <= |x| < hi and scientific
+ *     otherwise, hi = 1e6 in style 0 and 1e16 in style 1 (both compared with the exact float32 value).  Positional text
+ *     always has a fraction digit ("100000.0", "-0.0"); scientific text drops a lone ".0" and has a signed exponent of
+ *     at least two digits ("1e+07", "1e-45", "3.4028235e+38"); "inf", "-inf", and "nan" for every NaN bit pattern.
+ *
+ * b2r_rec_csv: users int64 [N], items int64 [N, k] and scores float32 [N, k] (row-major, row stride k), sep one ASCII
+ *   byte other than NUL, '"', CR and LF (anything else is B2R_E_BADARG).  Writes row r at out[row_offsets[r] ..
+ *   row_offsets[r + 1]) and the text's length at row_offsets[N] (row_offsets int64 [N + 1]); out must hold
+ *   b2r_rec_csv_text_bytes_max(N, k, style) bytes (every element at its longest text), else B2R_E_WORKSPACE.  One warp
+ *   per row measures the row, a scan places the rows, a second pass writes them: the output is a function of the inputs
+ *   alone.  Workspace b2r_rec_csv_workspace_bytes(N), 256-byte aligned; 0 <= N < 2^31 - 1, 0 <= k <= 65536.
+ * ---------------------------------------------------------------------------------------------- */
+#define B2R_REC_STYLE_NP 0
+#define B2R_REC_STYLE_BARE 1
+B2R_API size_t b2r_rec_csv_workspace_bytes(int64_t N);
+B2R_API size_t b2r_rec_csv_text_bytes_max(int64_t N, int k, int style);
+B2R_API int b2r_rec_csv(const int64_t* users, const int64_t* items, const float* scores, int64_t N, int k, int style,
+                        int sep, char* out, size_t out_capacity, int64_t* row_offsets, void* workspace,
+                        size_t workspace_bytes, b2r_stream_t stream);
+
+/* ------------------------------------------------------------------------------------------------
  * Impression evaluation and training batches (row f4): ImpressionRunner.evaluate (helpers/ImpressionRunner.py:135-171)
  * for the non-test_all branch on the device, batch by batch, without feed dicts or a host copy of the predictions; and
  * the batches and labels of ImpressionRunner.fit (:173-197) in the DataLoader's shuffled order.

@@ -165,6 +165,10 @@ SIGNATURES = {
     "b2r_topk_all_items": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p, C.c_int64, C.c_int, C.c_void_p, C.c_void_p,
                                      C.c_int, C.c_void_p, C.c_void_p, C.c_int64, C.c_int, C.c_void_p, C.c_void_p,
                                      C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p]),
+    "b2r_rec_csv_workspace_bytes": (C.c_size_t, [C.c_int64]),
+    "b2r_rec_csv_text_bytes_max": (C.c_size_t, [C.c_int64, C.c_int, C.c_int]),
+    "b2r_rec_csv": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_int, C.c_int, C.c_int, C.c_void_p,
+                              C.c_size_t, C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p]),
     "b2r_collate_impression": (C.c_int, [C.c_void_p] * 5 + [C.c_int64, C.c_int64, C.c_int, C.c_int, C.c_int,
                                                             C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
     "b2r_collate_impression_train": (C.c_int, [C.c_void_p] * 8 + [C.c_int64, C.c_int64, C.c_int, C.c_int, C.c_int,

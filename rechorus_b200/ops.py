@@ -367,6 +367,38 @@ def topk_all_items(q: torch.Tensor, table: torch.Tensor, target: torch.Tensor, u
     return items, scores
 
 
+REC_STYLE_NP, REC_STYLE_BARE = 0, 1          # B2R_REC_STYLE_*: np.int64(3) / np.float32(0.5), or 3 / 0.5
+
+
+def rec_csv_text_bytes_max(N: int, k: int, style: int) -> int:
+    """the longest text rec_csv can write for N rows of k elements in `style` (0 for a shape it refuses)"""
+    return int(_lib.load().b2r_rec_csv_text_bytes_max(int(N), int(k), int(style)))
+
+
+def rec_csv(users: torch.Tensor, items: torch.Tensor, scores: torch.Tensor, style: int, sep: str, out: torch.Tensor,
+            row_offsets: torch.Tensor) -> None:
+    """The rows of save_rec_results' CSV (include/b200rec.h, b2r_rec_csv): users int64 [N], items int64 [N, k], scores
+    float32 [N, k]; row r goes to out (uint8, at least rec_csv_text_bytes_max(N, k, style) bytes) at
+    [row_offsets[r], row_offsets[r + 1]), the text's length to row_offsets[N] (int64 [N + 1])."""
+    _need_cuda(users, items, scores, out, row_offsets)
+    users, items = _i64c(users.reshape(-1), "users"), _i64c(items, "items")
+    scores = _f32c(scores, "scores")
+    N = users.numel()
+    if items.dim() != 2 or scores.shape != items.shape or items.shape[0] != N:
+        raise ValueError("rec_csv: users [N], items [N, k] and scores [N, k]")
+    if out.dtype != torch.uint8 or not out.is_contiguous() or row_offsets.dtype != torch.int64 \
+            or not row_offsets.is_contiguous() or row_offsets.numel() < N + 1:
+        raise ValueError("rec_csv: out must be contiguous uint8, row_offsets contiguous int64 [N + 1]")
+    sep_b = sep.encode("utf-8") if isinstance(sep, str) else bytes(sep)
+    if len(sep_b) != 1:
+        raise ValueError(f"rec_csv: sep must be one byte, got {sep!r}")
+    L = _lib.load()
+    nb = L.b2r_rec_csv_workspace_bytes(N)
+    ws = _ws(nb, users.device)
+    _lib.check(L.b2r_rec_csv(_p(users), _p(items), _p(scores), N, items.shape[1], int(style), sep_b[0], _p(out),
+                             out.numel(), _p(row_offsets), _p(ws), nb, _stream()), "b2r_rec_csv")
+
+
 def neumf_all_items_error(d: int, layers: Sequence[int], Bn: int, n_items: int) -> Optional[str]:
     """None when NeuMF's test_all scores of a batch of Bn rows can come from neumf_score_rows (d in {32, 64}, at least
     4096 candidate rows, every hidden layer on the forward's tensor-core Linear, the fused CTA within shared memory), else

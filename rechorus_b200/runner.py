@@ -9,6 +9,7 @@ from __future__ import annotations
 import gc
 import logging
 import os
+from concurrent.futures import ThreadPoolExecutor
 from time import time
 from typing import Dict, List
 
@@ -315,6 +316,123 @@ def fit_impression_on_device(runner, dataset, epoch=-1) -> float:
     out = np.mean(losses.cpu().numpy()).item()
     _poll_ids(model)
     return out
+
+
+def recommend_batches(runner, dataset, k: int):
+    """Yields (first row, item ids int64 [Bn, k'], scores float32 [Bn, k']) on the device for every batch of an
+    evaluation phase, in dataset order: ``device_eval_batches``' batches through ``model.recommend``.  Each batch's
+    tensors are its own (later batches do not overwrite them).  The out-of-range-id poll runs after the last batch."""
+    model = dataset.model
+    model.eval()
+    start = 0
+    for feed, clicked in device_eval_batches(dataset, runner.eval_batch_size):
+        items, scores = model.recommend(feed, k, clicked)
+        yield start, items, scores
+        start += feed["batch_size"]
+    _poll_ids(model)
+
+
+_REC_PROBE = {"[np.int64(-3), np.float32(0.5), np.float32(1e-05)]": ops.REC_STYLE_NP,
+              "[-3, 0.5, 1e-05]": ops.REC_STYLE_BARE}
+
+
+def rec_csv_style(sep, users):
+    """The element style (ops.REC_STYLE_NP or ops.REC_STYLE_BARE) in which ``write_rec_csv`` writes the bytes pandas
+    writes for save_rec_results, or None when only pandas should write them.  The device writer needs:
+      - NumPy printing scalars in one of the two styles the kernels implement: NumPy >= 2 without legacy printing
+        (np.int64(3), np.float32(0.5)), or NumPy 1.x or legacy='1.25' (3, 0.5) -- decided from the version and the
+        print options, and confirmed on a probe list (legacy='1.13', for one, formats float32 differently);
+      - a separator that is one ASCII character other than NUL, '"', CR and LF (pandas quotes with '"' and ends lines
+        with LF; any other single character only wraps the fields that contain it);
+      - integer user ids that fit int64 (or none: an empty phase writes the header alone)."""
+    legacy = np.get_printoptions()["legacy"]
+    major = int(np.__version__.split(".")[0])
+    if legacy is False:
+        want = ops.REC_STYLE_NP if major >= 2 else ops.REC_STYLE_BARE
+    elif legacy == "1.25":
+        want = ops.REC_STYLE_BARE
+    else:
+        return None
+    if _REC_PROBE.get(str([np.int64(-3), np.float32(0.5), np.float32(1e-05)])) != want:
+        return None
+    if not isinstance(sep, str) or len(sep) != 1 or not 0 < ord(sep) < 128 or sep in "\"\r\n":
+        return None
+    u = np.asarray(users)
+    if (u.size and u.dtype.kind not in "iu") or (u.dtype == np.uint64 and u.size and int(u.max()) > np.iinfo(np.int64).max):
+        return None
+    return want
+
+
+REC_CSV_WINDOW_BYTES = 64 << 20      # device text of one window of save_rec_results' rows (and of each pinned copy)
+
+
+def _write_window(f, host: torch.Tensor, done) -> None:
+    done.synchronize()               # the window's copy to the pinned buffer has landed
+    f.write(memoryview(host.numpy()))
+
+
+def write_rec_csv(runner, dataset, result_path: str, topk: int, sep: str, style: int) -> None:
+    """save_rec_results' CSV written from the device (ops.rec_csv, include/b200rec.h): the header, then the rows of
+    ``recommend_batches`` in windows of W rows, W chosen so that a window's text fits REC_CSV_WINDOW_BYTES whatever the
+    phase's size.  Each batch's lists are staged into the window on the device, a full window is formatted, copied into
+    one of two pinned host buffers and written with one ``write`` by a writer thread, so the file write of window i
+    overlaps the lists, formatting and copy of window i + 1.  A call that fails removes the file it was writing."""
+    d = os.path.dirname(result_path)
+    if d:
+        os.makedirs(d, exist_ok=True)
+    users = _eval_state(dataset, int(runner.eval_batch_size))["users"]
+    dev = users.device
+    header = sep.join('"%s"' % c if sep in c else c for c in ("user_id", "rec_items", "rec_predictions")) + "\n"
+    st = {"rows": 0, "filled": 0, "window": 0, "pending": [None, None]}
+
+    def flush(ex, f):
+        n = st["filled"]
+        ops.rec_csv(users[st["rows"]:st["rows"] + n], st["items"][:n], st["scores"][:n], style, sep, st["text"],
+                    st["offsets"])
+        total = int(st["offsets"][n])
+        b = st["window"] % 2
+        if st["pending"][b] is not None:
+            st["pending"][b].result()                               # window i - 2 is written: its buffer is free
+        host = st["pinned"][b][:total]
+        host.copy_(st["text"][:total], non_blocking=True)
+        done = torch.cuda.Event()
+        done.record()
+        st["pending"][b] = ex.submit(_write_window, f, host, done)
+        st["rows"] += n
+        st["filled"] = 0
+        st["window"] += 1
+
+    try:
+        with open(result_path, "wb") as f, ThreadPoolExecutor(max_workers=1) as ex:
+            f.write(header.encode("ascii"))
+            for _, items, scores in recommend_batches(runner, dataset, topk):
+                if "W" not in st:
+                    kk = items.shape[1]
+                    row_max = ops.rec_csv_text_bytes_max(1, kk, style)
+                    W = st["W"] = max(1, min(users.numel(), REC_CSV_WINDOW_BYTES // row_max))
+                    st["items"] = torch.empty((W, kk), dtype=torch.int64, device=dev)
+                    st["scores"] = torch.empty((W, kk), dtype=torch.float32, device=dev)
+                    st["text"] = torch.empty(W * row_max, dtype=torch.uint8, device=dev)
+                    st["offsets"] = torch.empty(W + 1, dtype=torch.int64, device=dev)
+                    st["pinned"] = [torch.empty(W * row_max, dtype=torch.uint8, pin_memory=True) for _ in range(2)]
+                i, Bn = 0, items.shape[0]
+                while i < Bn:
+                    n = min(Bn - i, st["W"] - st["filled"])
+                    st["items"][st["filled"]:st["filled"] + n].copy_(items[i:i + n])
+                    st["scores"][st["filled"]:st["filled"] + n].copy_(scores[i:i + n])
+                    st["filled"] += n
+                    i += n
+                    if st["filled"] == st["W"]:
+                        flush(ex, f)
+            if st["filled"]:
+                flush(ex, f)
+            for p in st["pending"]:
+                if p is not None:
+                    p.result()
+    except BaseException:
+        if os.path.exists(result_path):
+            os.remove(result_path)
+        raise
 
 
 class BaseRunner:
@@ -752,22 +870,23 @@ class BaseRunner:
         arrays, rows in dataset order.  The batches are evaluate_on_device's (``device_eval_batches``); under test_all a
         dot-product model scores the catalogue itself (ops.topk_all_items) and NeuMF's [target | arange(1, n_items)]
         predictions are masked with ops.mask_clicked."""
-        model = dataset.model
-        model.eval()
         out_items, out_scores = [], []
-        for feed, clicked in device_eval_batches(dataset, self.eval_batch_size):
-            items, scores = model.recommend(feed, k, clicked)
+        for _, items, scores in recommend_batches(self, dataset, k):
             out_items.append(items)
             out_scores.append(scores)
-        _poll_ids(model)
         if not out_items:
             return list(dataset.data["user_id"]), np.zeros((0, 0), np.int64), np.zeros((0, 0), np.float32)
         return (list(dataset.data["user_id"]), torch.cat(out_items).cpu().numpy(), torch.cat(out_scores).cpu().numpy())
 
     def save_rec_results(self, dataset, result_path: str, topk: int = 100, sep: str = "\t") -> None:
-        """The TopK branch of main.py:117-132 (save_rec_results) with the lists from ``recommend``: same columns and
-        element types (NumPy int64 item ids, NumPy float32 scores), so the CSV matches the reference's byte for byte.
-        Writing the CSV stays on the host."""
+        """The TopK branch of main.py:117-132 (save_rec_results) with the lists from ``recommend``: the CSV matches the
+        reference's byte for byte.  When ``rec_csv_style`` says the device can write what pandas writes, the lists never
+        leave the device: ``write_rec_csv`` formats them there, window by window.  Otherwise the lists are written as the
+        reference writes them, a DataFrame of Python lists of NumPy scalars through pandas' to_csv."""
+        style = rec_csv_style(sep, dataset.data["user_id"])
+        if style is not None:
+            write_rec_csv(self, dataset, result_path, topk, sep, style)
+            return
         import pandas as pd
         users, items, scores = self.recommend(dataset, topk)
         d = os.path.dirname(result_path)
