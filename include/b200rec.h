@@ -341,6 +341,30 @@ B2R_API int b2r_attention_last_fwd(const float* q_last, const float* k, const fl
 B2R_API int b2r_attention_last_bwd(const float* q_last, const float* k, const float* v, int ld, const int64_t* lengths,
                                    const float* prob, const float* dctx_last, float* dq_last, float* dk, float* dv,
                                    int ldg, int B, int L, int d, int H, b2r_stream_t stream);
+/* Tiled causal attention (csrc/attention_tiled.cu): the function of b2r_attention_fwd/bwd_rt, with the same lse and the
+ * same dead-row contract (rows >= live[b] of ctx / dq / dk / dv written as zeros), for batch widths the shared-memory
+ * kernels cannot hold: key/value (forward, dQ) and query/dO/(lse, delta) (dK/dV) tiles of one head stream through a
+ * fixed-size shared-memory ring, so L may reach 65535 (the dropout masks' position field).  Covers d/H in {8, 16, 32, 64},
+ * d <= 256, d, ld and ldg multiples of 4, 16-byte aligned pointers; anything else returns B2R_E_UNSUPPORTED.
+ * Bit identity: wherever b2r_attention_fwd_rt / _bwd_rt accept a shape, ctx, lse, dq, dk and dv are the same bits (each
+ * lane runs the rt kernels' sequence of operations; only the staging differs).  d/H = 64 splits a row over two lanes.
+ * The backward takes a caller workspace of b2r_attention_bwd_tiled_workspace_bytes(B, L, H) bytes (delta = dO . O per
+ * row and head; may be NULL when B = 0); it allocates nothing, so both directions can be captured in a CUDA graph. */
+B2R_API size_t b2r_attention_bwd_tiled_workspace_bytes(int B, int L, int H);
+B2R_API int b2r_attention_fwd_tiled(const float* q, const float* k, const float* v, int ld, const int64_t* live, float* ctx,
+                                    float* lse, int B, int L, int d, int H, b2r_stream_t stream);
+B2R_API int b2r_attention_bwd_tiled(const float* q, const float* k, const float* v, int ld, const int64_t* live,
+                                    const float* ctx, const float* lse, const float* dctx, float* dq, float* dk, float* dv,
+                                    int ldg, int B, int L, int d, int H, void* ws, size_t ws_bytes, b2r_stream_t stream);
+/* The last-query form for 1 <= L <= 65535: arguments and results of b2r_attention_last_fwd / _bwd, the same bits wherever
+ * those accept a shape (L <= 256).  The score row lives in prob (forward) or in a workspace row per (sequence, head)
+ * (backward, b2r_attention_bwd_tiled_workspace_bytes(B, L, H) bytes) instead of shared memory. */
+B2R_API int b2r_attention_last_fwd_tiled(const float* q_last, const float* k, const float* v, int ld, const int64_t* lengths,
+                                         float* ctx_last, float* prob, int B, int L, int d, int H, b2r_stream_t stream);
+B2R_API int b2r_attention_last_bwd_tiled(const float* q_last, const float* k, const float* v, int ld, const int64_t* lengths,
+                                         const float* prob, const float* dctx_last, float* dq_last, float* dk, float* dv,
+                                         int ldg, int B, int L, int d, int H, void* ws, size_t ws_bytes,
+                                         b2r_stream_t stream);
 B2R_API int b2r_select_last(const float* y, const int64_t* hist, const int64_t* lengths, float* h, int B, int L,
                     int d, b2r_stream_t stream);
 B2R_API int b2r_select_last_bwd(const float* dh, const int64_t* hist, const int64_t* lengths, float* dy, int B, int L,
@@ -359,6 +383,10 @@ B2R_API int b2r_small_table_grad(const float* src, int ld, const int64_t* ids, i
  * (b2r_attention_last_*); any other flag bit is B2R_E_BADARG.  Host only: no device call is made. */
 #define B2R_SEQ_LAST_QUERY 1
 B2R_API int b2r_seq_train_check(int L, int d, int H, int full_blocks, int flags);
+/* The same question when widths the default kernels refuse may run on the tiled ones (b2r_attention_*_tiled, the
+ * --tiled_attention switch): accepts everything b2r_seq_train_check accepts and, beyond it, every L <= 65535 at d <= 256
+ * with d/H in {8, 16, 32, 64}; monotone in L.  Refusals name the kernel and limit as b2r_seq_train_check's do. */
+B2R_API int b2r_seq_train_check_tiled(int L, int d, int H, int full_blocks, int flags);
 
 /* out[r,k] = a[r,k] * w[k]   and   out[k] = sum_r a[r,k] * b[r,k]   (the GMF half of NeuMF's final Linear,
  * models/general/NeuMF.py:68,74-75, and its weight gradient) */

@@ -46,3 +46,26 @@ extern "C" int b2r_seq_train_check(int L, int d, int H, int full_blocks, int fla
         }
     return 0;
 }
+
+// The envelope with --tiled_attention: what b2r_seq_train_check accepts runs on the same kernels; the rest may run on the
+// tiled kernels (attention_tiled.cu) and the long last-query form (attention_last.cu, *_tiled), whose shared memory does
+// not depend on L.  A superset of b2r_seq_train_check, monotone in L.
+extern "C" int b2r_seq_train_check_tiled(int L, int d, int H, int full_blocks, int flags) {
+    B2R_REQUIRE(L > 0 && d > 0 && d % 4 == 0 && H > 0 && d % H == 0 && full_blocks >= 0 &&
+                    (flags & ~B2R_SEQ_LAST_QUERY) == 0,
+                B2R_E_BADARG, "b2r_seq_train_check_tiled: bad arguments L=%d d=%d H=%d full_blocks=%d flags=%d", L, d, H,
+                full_blocks, flags);
+    if (b2r_seq_train_check(L, d, H, full_blocks, flags) == 0) return 0;
+    B2R_REQUIRE(d <= kLNMaxD, B2R_E_UNSUPPORTED, "b2r_add_layernorm_bwd: d=%d, the kernel needs d <= %d", d, kLNMaxD);
+    B2R_REQUIRE(L <= kTiledMaxL, B2R_E_UNSUPPORTED,
+                "b2r_dropout: batch width L=%d, the masks' 16-bit position field needs L <= %d", L, kTiledMaxL);
+    // a batch may be narrower than L: widths the default kernels take run on them, every other width on the tiled ones
+    if (full_blocks > 0 && !tiled_shape_ok(L, d, H, d))
+        for (int l = 1; l <= L; ++l) {
+            if (full_attention_check(l, d, H) == 0) continue;
+            return b2r::set_error(B2R_E_UNSUPPORTED,
+                                  "b2r_attention_fwd_tiled / _bwd_tiled: head width d/H=%d at batch width L=%d, the kernels "
+                                  "need d/H in {8, 16, 32, 64} (the shared-memory kernels stop at L=%d)", d / H, l, l - 1);
+        }
+    return 0;
+}

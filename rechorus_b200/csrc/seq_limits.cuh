@@ -1,6 +1,7 @@
 // seq_limits.cuh -- shape limits of SASRec's sequence kernels, in one place: the launchers (attention.cu, attention_rt.cu,
-// attention_last.cu, dense.cu) refuse with these predicates and b2r_seq_train_check (seq_check.cu) answers from them, so
-// the construction-time check and the kernels cannot disagree.
+// attention_last.cu, attention_tiled.cu, dense.cu) refuse with these predicates and b2r_seq_train_check /
+// b2r_seq_train_check_tiled (seq_check.cu) answer from them, so the construction-time check and the kernels cannot
+// disagree.
 #pragma once
 #include <stddef.h>
 
@@ -21,6 +22,21 @@ static inline bool rt_shape_ok(int L, int d, int H, int ld) {
 static inline size_t rt_fwd_smem(int L, int d) { return (size_t)3 * L * (d + 4) * sizeof(float); }
 static inline size_t rt_bwd_smem(int L, int d, int H) {
     return ((size_t)5 * L * (d + 4) + (size_t)2 * L * H) * sizeof(float);
+}
+
+// tiled attention (attention_tiled.cu) and the long last-query form (attention_last.cu): shared memory does not depend
+// on L.  The batch width stops where the dropout masks' 16-bit position field does (dropout.cuh, check_dropout).
+constexpr int kTiledMaxL = 65535;
+
+static inline bool tiled_shape_ok(int L, int d, int H, int ld) {
+    if (H <= 0 || d % H != 0) return false;
+    const int dk = d / H;
+    return (dk == 8 || dk == 16 || dk == 32 || dk == 64) && L >= 1 && L <= kTiledMaxL && d <= kLNMaxD && d % 4 == 0 &&
+           ld % 4 == 0;
+}
+
+static inline bool tiled_last_shape_ok(int L, int d, int H) {
+    return H > 0 && d % H == 0 && L >= 1 && L <= kTiledMaxL;
 }
 
 // shared-memory operand attention (attention.cu)

@@ -142,12 +142,23 @@ SIGNATURES = {
                                        C.c_int, C.c_int, C.c_int, C.c_int, C.c_void_p]),
     "b2r_attention_bwd_rt": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int] + [C.c_void_p] * 7 +
                              [C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_void_p]),
+    "b2r_attention_bwd_tiled_workspace_bytes": (C.c_size_t, [C.c_int, C.c_int, C.c_int]),
+    "b2r_attention_fwd_tiled": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p,
+                                          C.c_int, C.c_int, C.c_int, C.c_int, C.c_void_p]),
+    "b2r_attention_bwd_tiled": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int] + [C.c_void_p] * 7 +
+                                [C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_size_t, C.c_void_p]),
+    "b2r_attention_last_fwd_tiled": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p,
+                                               C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_void_p]),
+    "b2r_attention_last_bwd_tiled": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p,
+                                               C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int,
+                                               C.c_int, C.c_int, C.c_void_p, C.c_size_t, C.c_void_p]),
     "b2r_select_last": (C.c_int, [C.c_void_p] * 4 + [C.c_int, C.c_int, C.c_int, C.c_void_p]),
     "b2r_select_last_bwd": (C.c_int, [C.c_void_p] * 4 + [C.c_int, C.c_int, C.c_int, C.c_void_p]),
     "b2r_small_table_grad_workspace_bytes": (C.c_size_t, [C.c_int64, C.c_int, C.c_int]),
     "b2r_small_table_grad": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p, C.c_int64, C.c_int, C.c_int, C.c_void_p,
                                        C.c_void_p, C.c_size_t, C.c_void_p]),
     "b2r_seq_train_check": (C.c_int, [C.c_int, C.c_int, C.c_int, C.c_int, C.c_int]),
+    "b2r_seq_train_check_tiled": (C.c_int, [C.c_int, C.c_int, C.c_int, C.c_int, C.c_int]),
     "b2r_colscale": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_int, C.c_void_p]),
     "b2r_gt_rank": (C.c_int, [C.c_void_p, C.c_int64, C.c_int64, C.c_int64, C.c_void_p, C.c_void_p]),
     "b2r_rank_histogram": (C.c_int, [C.c_void_p, C.c_int64, C.c_int, C.c_void_p, C.c_void_p]),

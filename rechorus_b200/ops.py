@@ -14,6 +14,7 @@ Embedding-table gradients can leave the autograd graph in three forms, selected 
 from __future__ import annotations
 
 import ctypes as C
+import functools
 from dataclasses import dataclass
 from typing import List, Optional, Sequence, Tuple
 
@@ -1401,12 +1402,32 @@ def add_layernorm(x, res, gamma, beta, eps=1e-5, drop: Optional[Drop] = None, le
     return _AddLayerNorm.apply(x, res, gamma, beta, eps, drop, lengths, int(seq_len))
 
 
+@functools.lru_cache(maxsize=None)
+def _tiled_route(Ln: int, d: int, H: int, last_query: bool) -> bool:
+    """Whether attention of batch width Ln runs on the tiled kernels when tiled=True: only when the default kernels refuse
+    the shape (forward and backward) and the tiled ones take it -- the keyword admits shapes, it never chooses between
+    two kernels for one input.  Answered by the library's envelope checks, so it agrees with the launchers."""
+    L_ = _lib.load()
+    blocks, flags = (0, _lib.SEQ_LAST_QUERY) if last_query else (1, 0)
+    return (L_.b2r_seq_train_check(Ln, d, H, blocks, flags) != 0
+            and L_.b2r_seq_train_check_tiled(Ln, d, H, blocks, flags) == 0)
+
+
+def _tiled_workspace(B: int, Ln: int, H: int, device) -> torch.Tensor:
+    return torch.empty(int(_lib.load().b2r_attention_bwd_tiled_workspace_bytes(B, Ln, H)), dtype=torch.uint8,
+                       device=device)
+
+
 class _CausalAttention(torch.autograd.Function):
     """layers.py:52-63 for q,k,v [B, L, d] with H heads (contiguous d/H chunks), causal mask, no W_o.  ``live`` (optional
-    int64 [B]): positions >= live[b] are dead rows (nothing downstream reads them): skipped, written as zeros."""
+    int64 [B]): positions >= live[b] are dead rows (nothing downstream reads them): skipped, written as zeros.
+    ``tiled``: widths the register-resident and shared-memory kernels refuse run on the tiled ones (csrc/attention_tiled.cu).
+    The route is chosen for forward and backward together: a width whose backward only the tiled kernels take runs its
+    forward on them too (even where b2r_attention_fwd_live alone would accept it, e.g. L = 200, d = 64, H = 4), because
+    the tiled backward needs the forward's lse, and so a no-grad evaluation gives the same bits as a training forward."""
 
     @staticmethod
-    def forward(ctx, q, k, v, H, live):
+    def forward(ctx, q, k, v, H, live, tiled):
         _need_cuda(q, k, v, live)
         B, Ln, d = q.shape
         q, k, v = _f32c(q, "q"), _f32c(k, "k"), _f32c(v, "v")
@@ -1414,7 +1435,12 @@ class _CausalAttention(torch.autograd.Function):
         out = torch.empty((B, Ln, d), dtype=torch.float32, device=q.device)
         L = _lib.load()
         lse = None
-        if d % H == 0 and d // H in (8, 16, 32) and Ln <= 128:
+        ctx.tiled = bool(tiled) and _tiled_route(Ln, d, H, False)
+        if ctx.tiled:
+            lse = torch.empty((B, Ln, H), dtype=torch.float32, device=q.device)
+            _lib.check(L.b2r_attention_fwd_tiled(_p(q), _p(k), _p(v), d, _p(live), _p(out), _p(lse), B, Ln, d, H, _stream()),
+                       "b2r_attention_fwd_tiled")
+        elif d % H == 0 and d // H in (8, 16, 32) and Ln <= 128:
             # register-resident kernels (csrc/attention_rt.cu); the row log-sum-exp is kept for the backward
             lse = torch.empty((B, Ln, H), dtype=torch.float32, device=q.device)
             rc = L.b2r_attention_fwd_rt(_p(q), _p(k), _p(v), d, _p(live), _p(out), _p(lse), B, Ln, d, H, _stream())
@@ -1436,43 +1462,53 @@ class _CausalAttention(torch.autograd.Function):
         dout = _f32c(dout, "dctx")
         dq, dk, dv = torch.empty_like(q), torch.empty_like(q), torch.empty_like(q)
         L = _lib.load()
-        if lse is not None:
+        if ctx.tiled:
+            ws = _tiled_workspace(B, Ln, ctx.H, q.device)
+            _lib.check(L.b2r_attention_bwd_tiled(_p(q), _p(k), _p(v), d, _p(live), _p(out), _p(lse), _p(dout), _p(dq),
+                                                 _p(dk), _p(dv), d, B, Ln, d, ctx.H, _p(ws), ws.numel(), _stream()),
+                       "b2r_attention_bwd_tiled")
+        elif lse is not None:
             _lib.check(L.b2r_attention_bwd_rt(_p(q), _p(k), _p(v), d, _p(live), _p(out), _p(lse), _p(dout), _p(dq), _p(dk),
                                               _p(dv), d, B, Ln, d, ctx.H, _stream()), "b2r_attention_bwd_rt")
         else:
             _lib.check(L.b2r_attention_bwd_live(_p(q), _p(k), _p(v), d, _p(live), _p(dout), _p(dq), _p(dk), _p(dv), d, B, Ln,
                                                 d, ctx.H, _stream()), "b2r_attention_bwd_live")
-        return dq, dk, dv, None, None
+        return dq, dk, dv, None, None, None
 
 
-def causal_attention(q, k, v, num_heads, live=None):
-    return _CausalAttention.apply(q, k, v, num_heads, live)
+def causal_attention(q, k, v, num_heads, live=None, tiled=False):
+    return _CausalAttention.apply(q, k, v, num_heads, live, tiled)
 
 
-def seq_train_error(L: int, d: int, H: int, num_layers: int, last_query: bool) -> Optional[str]:
-    """None when a SASRec training step on batches of width up to L runs on the kernels (b2r_seq_train_check), else the
-    library's reason.  last_query: the last block runs for the one query per sequence (attention_last)."""
+def seq_train_error(L: int, d: int, H: int, num_layers: int, last_query: bool, tiled: bool = False) -> Optional[str]:
+    """None when a SASRec training step on batches of width up to L runs on the kernels (b2r_seq_train_check, or
+    b2r_seq_train_check_tiled when ``tiled``), else the library's reason.  last_query: the last block runs for the one
+    query per sequence (attention_last)."""
     last_query = bool(last_query) and num_layers > 0
     flags = _lib.SEQ_LAST_QUERY if last_query else 0
     L_ = _lib.load()
-    rc = L_.b2r_seq_train_check(int(L), int(d), int(H), int(num_layers) - int(last_query), flags)
+    check = L_.b2r_seq_train_check_tiled if tiled else L_.b2r_seq_train_check
+    rc = check(int(L), int(d), int(H), int(num_layers) - int(last_query), flags)
     return None if rc == 0 else L_.b2r_last_error().decode("utf-8", "replace")
 
 
 class _AttentionLast(torch.autograd.Function):
     """Attention for the one query per sequence that SASRec's last block needs (position len-1): q_last [B, d] against
-    k, v [B, L, d]; identical to row len-1 of _CausalAttention.  SASRec's last block runs on it; L <= 256."""
+    k, v [B, L, d]; identical to row len-1 of _CausalAttention.  SASRec's last block runs on it; L <= 256, or up to 65535
+    with ``tiled`` (the *_tiled entry points, for the widths the others refuse)."""
 
     @staticmethod
-    def forward(ctx, q_last, k, v, lengths, H):
+    def forward(ctx, q_last, k, v, lengths, H, tiled):
         _need_cuda(q_last, k, v, lengths)
         B, Ln, d = k.shape
         q_last, k, v = _f32c(q_last, "q_last"), _f32c(k, "k"), _f32c(v, "v")
         lengths = _i64c(lengths, "lengths")
         out = torch.empty((B, d), dtype=torch.float32, device=k.device)
         prob = torch.empty((B, H, Ln), dtype=torch.float32, device=k.device)
-        _lib.check(_lib.load().b2r_attention_last_fwd(_p(q_last), _p(k), _p(v), d, _p(lengths), _p(out), _p(prob), B, Ln,
-                                                      d, H, _stream()), "b2r_attention_last_fwd")
+        ctx.tiled = bool(tiled) and _tiled_route(Ln, d, H, True)
+        name = "b2r_attention_last_fwd_tiled" if ctx.tiled else "b2r_attention_last_fwd"
+        _lib.check(getattr(_lib.load(), name)(_p(q_last), _p(k), _p(v), d, _p(lengths), _p(out), _p(prob), B, Ln, d, H,
+                                              _stream()), name)
         ctx.save_for_backward(q_last, k, v, lengths, prob)
         ctx.H = H
         return out
@@ -1483,14 +1519,20 @@ class _AttentionLast(torch.autograd.Function):
         B, Ln, d = k.shape
         dout = _f32c(dout, "dctx_last")
         dq, dk, dv = torch.empty_like(q_last), torch.empty_like(k), torch.empty_like(k)
-        _lib.check(_lib.load().b2r_attention_last_bwd(_p(q_last), _p(k), _p(v), d, _p(lengths), _p(prob), _p(dout), _p(dq),
-                                                      _p(dk), _p(dv), d, B, Ln, d, ctx.H, _stream()),
-                   "b2r_attention_last_bwd")
-        return dq, dk, dv, None, None
+        L = _lib.load()
+        if ctx.tiled:
+            ws = _tiled_workspace(B, Ln, ctx.H, k.device)
+            _lib.check(L.b2r_attention_last_bwd_tiled(_p(q_last), _p(k), _p(v), d, _p(lengths), _p(prob), _p(dout), _p(dq),
+                                                      _p(dk), _p(dv), d, B, Ln, d, ctx.H, _p(ws), ws.numel(), _stream()),
+                       "b2r_attention_last_bwd_tiled")
+        else:
+            _lib.check(L.b2r_attention_last_bwd(_p(q_last), _p(k), _p(v), d, _p(lengths), _p(prob), _p(dout), _p(dq),
+                                                _p(dk), _p(dv), d, B, Ln, d, ctx.H, _stream()), "b2r_attention_last_bwd")
+        return dq, dk, dv, None, None, None
 
 
-def attention_last(q_last, k, v, lengths, num_heads):
-    return _AttentionLast.apply(q_last, k, v, lengths, num_heads)
+def attention_last(q_last, k, v, lengths, num_heads, tiled=False):
+    return _AttentionLast.apply(q_last, k, v, lengths, num_heads, tiled)
 
 
 class _EmbedHistory(torch.autograd.Function):

@@ -415,6 +415,8 @@ class SASRecKernels(_KernelModelMixin):
         parser.add_argument("--num_heads", type=int, default=4, help="Number of attention heads.")
         parser.add_argument("--table_mode", type=str, default="dense",
                             help="embedding gradient form: dense | sparse | fused (see rechorus_b200.ops)")
+        parser.add_argument("--tiled_attention", type=int, default=0,
+                            help="1: admit history widths the default attention kernels refuse, on the tiled kernels")
         return parser
 
     def _base_init(self, args, corpus):
@@ -423,14 +425,19 @@ class SASRecKernels(_KernelModelMixin):
         self.max_his = args.history_max
         self.num_layers = args.num_layers
         self.num_heads = args.num_heads
+        self.tiled_attention = bool(getattr(args, "tiled_attention", 0))
         if self.emb_size % 4 != 0 or self.emb_size % self.num_heads != 0:
             raise ValueError("rechorus_b200 kernels need emb_size % 4 == 0 and emb_size % num_heads == 0")
         if self.max_his > 0:
             # refused here rather than by the first backward (DESIGN.md, a8-a10: the trainable envelope)
-            err = ops.seq_train_error(self.max_his, self.emb_size, self.num_heads, self.num_layers, _SASREC_LASTQ)
+            shape = (self.max_his, self.emb_size, self.num_heads, self.num_layers, _SASREC_LASTQ)
+            err = ops.seq_train_error(*shape, tiled=self.tiled_attention)
             if err is not None:
+                hint = ""
+                if not self.tiled_attention and ops.seq_train_error(*shape, tiled=True) is None:
+                    hint = "; --tiled_attention 1 runs this shape on the tiled attention kernels"
                 raise ValueError(f"SASRec cannot train with history_max={self.max_his}, emb_size={self.emb_size}, "
-                                 f"num_heads={self.num_heads}, num_layers={self.num_layers} on these kernels: {err}")
+                                 f"num_heads={self.num_heads}, num_layers={self.num_layers} on these kernels: {err}{hint}")
         ops.check_dropout_p(self.dropout)                    # the reference's nn.Dropout(dropout) (layers.py:104,110)
         self._dropout_init()
         self._base_define_params()
@@ -461,7 +468,7 @@ class SASRecKernels(_KernelModelMixin):
         q_last = ops.linear(x_last, a.q_linear.weight, a.q_linear.bias)
         k = ops.linear(x, a.k_linear.weight, a.k_linear.bias)
         v = ops.linear(x, a.v_linear.weight, a.v_linear.bias)
-        ctx_last = ops.attention_last(q_last, k, v, lengths, self.num_heads)
+        ctx_last = ops.attention_last(q_last, k, v, lengths, self.num_heads, tiled=self.tiled_attention)
         c = ops.add_layernorm(ctx_last, x_last, blk.layer_norm1.weight, blk.layer_norm1.bias, drop=d1, lengths=lengths,
                               seq_len=Lb)
         o = ops.linear(ops.linear(c, blk.linear1.weight, blk.linear1.bias, relu=True), blk.linear2.weight, blk.linear2.bias)
@@ -485,7 +492,7 @@ class SASRecKernels(_KernelModelMixin):
             v = ops.linear(x, a.v_linear.weight, a.v_linear.bias)
             # rows at positions >= len are dead work (the model reads position len-1 only, SASRec.py:74-81, and the
             # mask is causal): skipped exactly
-            ctx = ops.causal_attention(q, k, v, self.num_heads, live=lengths)
+            ctx = ops.causal_attention(q, k, v, self.num_heads, live=lengths, tiled=self.tiled_attention)
             c = ops.add_layernorm(ctx, x, blk.layer_norm1.weight, blk.layer_norm1.bias, drop=d1)       # dropout1 fused
             o = ops.linear(ops.linear(c, blk.linear1.weight, blk.linear1.bias, relu=True),
                            blk.linear2.weight, blk.linear2.bias)
