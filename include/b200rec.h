@@ -422,9 +422,9 @@ B2R_API int b2r_collate_history(const int64_t* users, const int64_t* positions, 
                                 b2r_stream_t stream);
 
 /* ------------------------------------------------------------------------------------------------
- * Groundwork for the exact dense-Adam mode (not used by the default paths of this round): advance rows of a table whose
- * Adam state is kept row-sparsely through the optimizer steps they skipped, exactly as torch.optim.Adam over the whole
- * table (helpers/BaseRunner.py:110-114,206) would have moved them with a zero data gradient (g = weight_decay * w).
+ * The exact dense-Adam mode (--exact_adam 1): advance rows of a table whose Adam state is kept row-sparsely through the
+ * optimizer steps they skipped, exactly as torch.optim.Adam over the whole table (helpers/BaseRunner.py:110-114,206)
+ * would have moved them with a zero data gradient (g = weight_decay * w).  d in {32, 64, 128}.
  * last [n_rows] int32 holds the step each row is up to date with.  rows == NULL: all n_rows rows (flush); otherwise n
  * unique row ids.  Every processed row is brought to step `upto` and stamped max(upto, stamp) -- pass stamp = upto + 1
  * when the step-(upto+1) update with b2r_direct_plan_apply / b2r_segment_apply follows.  opt carries lr, betas, eps,
@@ -433,6 +433,17 @@ B2R_API int b2r_collate_history(const int64_t* users, const int64_t* positions, 
 B2R_API int b2r_adam_exact_advance(const int64_t* rows, int64_t n, int64_t n_rows, int d, float* W, float* m, float* v,
                                    int32_t* last, int upto, int stamp, const b2r_optim* opt, int32_t* err_flag,
                                    b2r_stream_t stream);
+/* The same advance over the raw ids a forward reads or an update writes (ids [n] int64, every repeat kept; e.g. a
+ * batch's [B] user ids, [B, C] candidate ids or [B, L] right-padded histories), deduplicated on the device with no sort
+ * and no host round trip: the stamp word is the claim.  For each id one atomicMax raises last[id] to max(upto, stamp);
+ * the one caller that finds it below `upto` advances the row from the stamp it found, all others leave it.  The result
+ * is the same bits as b2r_adam_exact_advance over the unique ids, whichever caller wins.  Positions [0, ignore_n) whose
+ * id equals ignore_id are skipped (the padding rule of b2r_direct_plan_build); out-of-range ids are skipped and counted
+ * in err_flag.  Ordered on `stream` after the writes of earlier launches, like any kernel: a forward enqueued behind it
+ * reads caught-up rows. */
+B2R_API int b2r_adam_exact_catch_up(const int64_t* ids, int64_t n, int64_t ignore_id, int64_t ignore_n, int64_t n_rows,
+                                    int d, float* W, float* m, float* v, int32_t* last, int upto, int stamp,
+                                    const b2r_optim* opt, int32_t* err_flag, b2r_stream_t stream);
 
 /* ------------------------------------------------------------------------------------------------
  * Evaluation (row f2): integer ranks of the ground-truth item on the device.
@@ -694,6 +705,13 @@ B2R_API int b2r_bprmf_ctx_reset(void* ctx);
  * `ctas` CTAs (0: grids sized to the work) on a side stream of the highest (high_priority != 0) or the default priority.
  * The defaults were measured on an H100 at the BASELINE config 2 shape; this entry point is for measuring others. */
 B2R_API int b2r_bprmf_ctx_plan_launch(void* ctx, int ctas, int high_priority);
+/* exact dense-Adam mode of the steps that follow (see b2r_adam_exact_catch_up): last_u [n_users] / last_i [n_items] are the
+ * tables' int32 stamps and `step` (>= 1) the optimizer step the next b2r_bprmf_train_step applies.  That step then first
+ * advances every row its ids read to step - 1 and stamps it `step` (one b2r_adam_exact_catch_up per table on the step's
+ * stream, before the forward), so the forward reads and the update moves rows that stand where dense torch.optim.Adam
+ * would have them.  opt's weight decay and state_ld serve both.  Call it before every exact step (the step count is
+ * the caller's); last_u = last_i = NULL returns the context to the lazy rule. */
+B2R_API int b2r_bprmf_ctx_exact(void* ctx, int32_t* last_u, int32_t* last_i, int step);
 B2R_API int b2r_bprmf_train_step(void* ctx, const b2r_bprmf_tables* t, const int64_t* uid, const int64_t* iid,
                          const int64_t* next_uid, const int64_t* next_iid, const b2r_optim* opt,
                          float* loss_out, int32_t* err_flag, b2r_stream_t stream);

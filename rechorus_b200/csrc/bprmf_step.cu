@@ -1,7 +1,8 @@
 // bprmf_step.cu -- one whole BPRMF training step enqueued from C (b2r_bprmf_train_step) on a step context.
 //
 // Stream plan (step t):
-//   main :  fused gather+score+loss+dQ (rows read once) -> mean(loss) -> [wait plan(t)] -> opt(I) + opt(U) in one launch
+//   main :  [exact dense-Adam mode: catch-up(U), catch-up(I)] -> fused gather+score+loss+dQ (rows read once) -> mean(loss)
+//           -> [wait plan(t)] -> opt(I) + opt(U) in one launch
 //   side :  plan(t+1) for the NEXT batch's ids (or plan(t) itself when nothing was prefetched)
 // The index plan (per-bucket sort of the ids) only depends on the ids, so the context builds it one step ahead on
 // a library-owned non-blocking stream while the HBM-bound kernels of the current step run; joins are event
@@ -19,6 +20,9 @@ int b2r_bprmf_fused_fwd_bwd_loss(const float* U, const int64_t* uid, int64_t n_u
                                  int64_t n_items, float* grad_pred, float* row_loss, float* dQ, float* qout, int B, int C,
                                  int d, int32_t* err_flag, float* loss_out, unsigned int* done_counter,
                                  b2r_stream_t stream);
+int b2r_adam_exact_catch_up(const int64_t* ids, int64_t n, int64_t ignore_id, int64_t ignore_n, int64_t n_rows, int d,
+                            float* W, float* m, float* v, int32_t* last, int upto, int stamp, const b2r_optim* opt,
+                            int32_t* err_flag, b2r_stream_t stream);
 
 namespace b2r {
 
@@ -75,6 +79,9 @@ struct StepCtx {
     const void* pre_uid;
     const void* pre_iid;
     bool have_pre;
+    int32_t* last_u;                  // exact dense-Adam stamps (b2r_bprmf_ctx_exact); NULL: lazy row-sparse Adam
+    int32_t* last_i;
+    int exact_step;                   // the optimizer step the next train_step applies
 };
 
 // the plan stream, at the highest or the default priority (kPlanHighPriority)
@@ -116,6 +123,8 @@ extern "C" int b2r_bprmf_ctx_create(void** ctx_out, int B, int C, int d, int64_t
     c->slot = 0;
     c->have_pre = false;
     c->pre_uid = c->pre_iid = nullptr;
+    c->last_u = c->last_i = nullptr;
+    c->exact_step = 0;
     c->plan_ctas = kPlanCtas;
     c->plan_high = kPlanHighPriority;
     cudaError_t e = create_side_stream(c);
@@ -185,6 +194,17 @@ extern "C" int b2r_bprmf_ctx_reset(void* ctx) {
     return 0;
 }
 
+extern "C" int b2r_bprmf_ctx_exact(void* ctx, int32_t* last_u, int32_t* last_i, int step) {
+    B2R_REQUIRE(ctx, B2R_E_BADARG, "b2r_bprmf_ctx_exact: null context");
+    B2R_REQUIRE((last_u == nullptr) == (last_i == nullptr), B2R_E_BADARG, "b2r_bprmf_ctx_exact: pass both stamp arrays or neither");
+    B2R_REQUIRE(!last_u || step >= 1, B2R_E_BADARG, "b2r_bprmf_ctx_exact: step %d < 1", step);
+    StepCtx* c = static_cast<StepCtx*>(ctx);
+    c->last_u = last_u;
+    c->last_i = last_i;
+    c->exact_step = last_u ? step : 0;
+    return 0;
+}
+
 static int build_plans(StepCtx* c, int slot, const int64_t* uid, const int64_t* iid, int32_t* err_flag) {
     char* base = c->ws;
     const int64_t n = (int64_t)c->B * c->C;
@@ -236,6 +256,18 @@ extern "C" int b2r_bprmf_train_step(void* ctx, const b2r_bprmf_tables* t, const 
     c->pre_uid = prefetch ? next_uid : nullptr;
     c->pre_iid = prefetch ? next_iid : nullptr;
     c->slot = cur ^ 1;
+
+    // exact dense-Adam mode: every row the step reads and updates is advanced through the steps it skipped (to t - 1)
+    // and stamped t before the forward reads it; the update below then applies step t to rows standing at t - 1
+    if (c->last_u) {
+        const int t_ = c->exact_step;
+        rc = b2r_adam_exact_catch_up(uid, B, -1, 0, t->n_users, d, t->U, t->Um, t->Uv, c->last_u, t_ - 1, t_, opt,
+                                     err_flag, main_s);
+        if (rc == 0)
+            rc = b2r_adam_exact_catch_up(iid, n, -1, 0, t->n_items, d, t->I, t->Im, t->Iv, c->last_i, t_ - 1, t_, opt,
+                                         err_flag, main_s);
+        if (rc != 0) return rc;
+    }
 
     // main: forward + loss + query-side backward; the gathered user rows are kept in q (the item gradient's source)
     float* q = reinterpret_cast<float*>(base + c->L.q);

@@ -193,6 +193,9 @@ SIGNATURES = {
     "b2r_neumf_score_rows": (C.c_int, [C.POINTER(NeumfRows), C.c_void_p, C.c_void_p]),
     "b2r_adam_exact_advance": (C.c_int, [C.c_void_p, C.c_int64, C.c_int64, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p,
                                          C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "b2r_adam_exact_catch_up": (C.c_int, [C.c_void_p, C.c_int64, C.c_int64, C.c_int64, C.c_int64, C.c_int, C.c_void_p,
+                                          C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_void_p,
+                                          C.c_void_p]),
     "b2r_sample_negatives": (C.c_int, [C.c_void_p, C.c_int64, C.c_int, C.c_void_p, C.c_void_p, C.c_int64, C.c_int64,
                                        C.c_uint64, C.c_uint32, C.c_void_p, C.c_void_p, C.c_void_p]),
     "b2r_collate_general": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_int, C.c_int,
@@ -230,6 +233,7 @@ SIGNATURES = {
     "b2r_bprmf_ctx_destroy": (C.c_int, [C.c_void_p]),
     "b2r_bprmf_ctx_reset": (C.c_int, [C.c_void_p]),
     "b2r_bprmf_ctx_plan_launch": (C.c_int, [C.c_void_p, C.c_int, C.c_int]),
+    "b2r_bprmf_ctx_exact": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int]),
     "b2r_bprmf_train_step": (C.c_int, [C.c_void_p, C.POINTER(BprmfTables), C.c_void_p, C.c_void_p, C.c_void_p,
                                        C.c_void_p, C.POINTER(Optim), C.c_void_p, C.c_void_p, C.c_void_p]),
 }

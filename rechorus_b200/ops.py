@@ -679,22 +679,47 @@ def impression_metrics(pred: torch.Tensor, pos_num: torch.Tensor, neg_num: torch
     return acc
 
 
-def adam_exact_advance(W: torch.Tensor, m: torch.Tensor, v: torch.Tensor, last: torch.Tensor, upto: int, opt,
-                       rows: Optional[torch.Tensor] = None, stamp: int = 0, state_ld: int = 0) -> None:
-    """Groundwork for the exact dense-Adam mode (b2r_adam_exact_advance): bring the listed unique rows (all rows when
-    ``rows`` is None) of a row-sparsely updated table to optimizer step ``upto``, as torch.optim.Adam over the whole
-    table would have moved them on zero data gradients.  ``last`` int32 [n_rows] is read and re-stamped."""
-    _need_cuda(W, m, v, last, rows)
+def _exact_optim(opt, state_ld: int) -> _lib.Optim:
+    return _lib.Optim(1, opt.lr, opt.betas[0], opt.betas[1], opt.eps, opt.weight_decay, 1.0, 1.0, state_ld)
+
+
+def _check_last(last: torch.Tensor) -> None:
     if last.dtype != torch.int32 or not last.is_contiguous():
         raise TypeError("last must be a contiguous int32 tensor")
+
+
+def adam_exact_advance(W: torch.Tensor, m: torch.Tensor, v: torch.Tensor, last: torch.Tensor, upto: int, opt,
+                       rows: Optional[torch.Tensor] = None, stamp: int = 0, state_ld: int = 0) -> None:
+    """Exact dense-Adam mode (b2r_adam_exact_advance): bring the listed unique rows (all rows when ``rows`` is None) of
+    a row-sparsely updated table to optimizer step ``upto``, as torch.optim.Adam over the whole table would have moved
+    them on zero data gradients.  ``last`` int32 [n_rows] is read and re-stamped."""
+    _need_cuda(W, m, v, last, rows)
+    _check_last(last)
     n = 0
     if rows is not None:
         rows = _i64c(rows.reshape(-1), "rows")
         n = rows.numel()
-    o = _lib.Optim(1, opt.lr, opt.betas[0], opt.betas[1], opt.eps, opt.weight_decay, 1.0, 1.0, state_ld)
     _lib.check(_lib.load().b2r_adam_exact_advance(_p(rows), n, W.shape[0], W.shape[1], _p(W), _p(m), _p(v), _p(last),
-                                                  int(upto), int(stamp), C.byref(o), _p(err_flag(W.device)), _stream()),
+                                                  int(upto), int(stamp), C.byref(_exact_optim(opt, state_ld)),
+                                                  _p(err_flag(W.device)), _stream()),
                "b2r_adam_exact_advance")
+
+
+def adam_exact_catch_up(W: torch.Tensor, m: torch.Tensor, v: torch.Tensor, last: torch.Tensor, ids: torch.Tensor,
+                        upto: int, opt, stamp: int = 0, ignore_id: int = -1, ignore_n: int = 0,
+                        state_ld: int = 0) -> None:
+    """b2r_adam_exact_catch_up: the advance of ``adam_exact_advance`` over raw ids with every repeat (any shape; a
+    forward's user, candidate or history ids), deduplicated on the device -- no sort, no host synchronisation.  Every
+    id's row ends at step ``upto`` and stamped max(upto, stamp); ids equal to ``ignore_id`` among the first
+    ``ignore_n`` positions are skipped (pass ``ignore_n = ids.numel()`` to skip them everywhere)."""
+    _need_cuda(W, m, v, last, ids)
+    _check_last(last)
+    ids = _i64c(ids.reshape(-1), "ids")
+    _lib.check(_lib.load().b2r_adam_exact_catch_up(_p(ids), ids.numel(), int(ignore_id), int(ignore_n), W.shape[0],
+                                                   W.shape[1], _p(W), _p(m), _p(v), _p(last), int(upto), int(stamp),
+                                                   C.byref(_exact_optim(opt, state_ld)), _p(err_flag(W.device)),
+                                                   _stream()),
+               "b2r_adam_exact_catch_up")
 
 
 def bpr_loss_and_grad(pred: torch.Tensor, want_grad: bool = True) -> Tuple[torch.Tensor, Optional[torch.Tensor]]:
@@ -1096,8 +1121,12 @@ def bprmf_train_step(U: torch.nn.Parameter, I: torch.nn.Parameter, optimizer, ui
             raise ValueError("prefetched id tensors must be contiguous int64 tensors that stay alive until the next step")
     else:
         next_uid = next_iid = None
-    optimizer.advance()
+    t = optimizer.advance()
     opt = optimizer._opt(ei["wd"], ei["state_ld"])
+    # exact dense-Adam mode: the step catches its rows up before its forward (b2r_bprmf_ctx_exact); reset for lazy steps
+    exact = "last" in eu and "last" in ei
+    _lib.check(L.b2r_bprmf_ctx_exact(ctx.handle, _p(eu["last"]) if exact else None, _p(ei["last"]) if exact else None,
+                                     t if exact else 0), "b2r_bprmf_ctx_exact")
     tables = _lib.BprmfTables(_p(U.data), _p(I.data), _p(eu["m"]), _p(eu["v"]), _p(ei["m"]), _p(ei["v"]),
                               U.shape[0], I.shape[0], d, 0)
     loss = torch.empty((), dtype=torch.float32, device=U.device)

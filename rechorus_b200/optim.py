@@ -8,7 +8,8 @@
   (b2r_segment_apply mode 2).  The update is *row-sparse / lazy*: rows the batch did not touch do not move.
   This is NOT what the reference's dense ``torch.optim.Adam`` does (there the moments keep moving untouched
   rows and L2 decays them every step); it is the semantics of ``torch.optim.SparseAdam`` and of production
-  recommender training.  Keep tables in 'dense' mode to reproduce the reference exactly.
+  recommender training.  Keep tables in 'dense' mode to reproduce the reference exactly, or pass ``exact_dense=True``
+  for the reference's dense Adam results at row-sparse cost.
 * every other parameter (and tables left in 'dense' mode) gets the exact dense torch.optim formula
   (b2r_dense_optim), with the reference's two parameter groups: names containing 'bias' have weight_decay 0
   (models/BaseModel.py:64-73).
@@ -29,10 +30,13 @@ _DEFAULT_EPS = {"SGD": 0.0, "Adam": 1e-8, "Adagrad": 1e-10}
 class RowSparseOptimizer:
     def __init__(self, model: torch.nn.Module, name: str = "Adam", lr: float = 1e-3, l2: float = 0.0,
                  betas=(0.9, 0.999), eps: float | None = None, exact_dense: bool = False, device_clock: bool = False):
-        """exact_dense (Adam only; next-round groundwork, not yet run on a GPU): keep the row-sparse cost but
-        reproduce the reference's dense torch.optim.Adam -- every fused table gets a per-row "up to date as of step"
-        stamp, rows are advanced through the steps they skipped before a forward reads them (``before_forward``)
-        and before they are updated, and ``flush()`` brings the whole table up to date (oracle.LazyExactAdam)."""
+        """exact_dense (Adam only): keep the row-sparse cost but reproduce the reference's dense torch.optim.Adam --
+        every fused table gets a per-row "up to date as of step" stamp, the rows a forward reads are advanced through
+        the steps they skipped before it reads them (``before_forward``, called by every kernel-backed model's
+        forward and by the single-call BPRMF step), the rows an update writes are stamped with its step, and
+        ``flush()`` brings the whole table up to date (oracle.LazyExactAdam).  The catch-up deduplicates the raw ids
+        on the device (b2r_adam_exact_catch_up), so the mode adds no host synchronisation to a training step.
+        Fused tables must be 32, 64 or 128 wide, the widths of the catch-up and apply kernels."""
         if name not in _KIND:
             raise ValueError(f"optimizer {name!r} not supported by the fused path (have {sorted(_KIND)})")
         if exact_dense and name != "Adam":
@@ -49,6 +53,7 @@ class RowSparseOptimizer:
         self.lr, self.l2, self.betas = float(lr), float(l2), (float(betas[0]), float(betas[1]))
         self.eps = _DEFAULT_EPS[name] if eps is None else float(eps)
         self.t = 0
+        self._flushed_at = 0                  # exact_dense: the step every row was last brought up to by flush()
         self.model = model
         self._entries: List[dict] = []
         for pname, p in model.named_parameters():
@@ -62,6 +67,9 @@ class RowSparseOptimizer:
                 mv = torch.zeros((p.shape[0], 2, p.shape[1]), dtype=p.dtype, device=p.device)
                 e["mv"], e["m"], e["v"], e["state_ld"] = mv, mv[:, 0, :], mv[:, 1, :], 2 * p.shape[1]
                 if self.exact_dense:
+                    if p.shape[1] not in (32, 64, 128):
+                        raise ValueError(f"exact_dense: table {pname} is {p.shape[1]} wide; the exact dense-Adam "
+                                         "catch-up runs on tables 32, 64 or 128 wide")
                     e["last"] = torch.zeros(p.shape[0], dtype=torch.int32, device=p.device)
             else:
                 if self.kind == _lib.OPT_ADAM:
@@ -71,27 +79,31 @@ class RowSparseOptimizer:
             self._entries.append(e)
 
     # -- exact dense-Adam bookkeeping (exact_dense=True) ----------------------------------------------------
-    def _advance(self, e: dict, rows, upto: int, stamp: int = 0) -> None:
+    def _cfg(self, e: dict):
         import types
-        cfg = types.SimpleNamespace(lr=self.lr, betas=self.betas, eps=self.eps, weight_decay=e["wd"])
-        ops.adam_exact_advance(e["p"].data, e["m"], e["v"], e["last"], upto, cfg, rows=rows, stamp=stamp,
-                               state_ld=e["state_ld"])
+        return types.SimpleNamespace(lr=self.lr, betas=self.betas, eps=self.eps, weight_decay=e["wd"])
 
-    def before_forward(self, param: torch.Tensor, ids: torch.Tensor) -> None:
-        """bring the rows a forward pass is about to read up to the current step (no-op unless exact_dense)"""
+    def before_forward(self, param: torch.Tensor, ids: torch.Tensor, ignore_id: int = -1) -> None:
+        """bring the rows a forward pass is about to read (``ids``, any shape, repeats allowed; ``ignore_id`` e.g. the
+        padding id of histories is skipped) up to the current step (no-op unless exact_dense)"""
         if not self.exact_dense:
             return
         e = self.entry(param)
         if "last" in e and self.t > 0:
-            self._advance(e, torch.unique(ids), self.t)
+            ops.adam_exact_catch_up(e["p"].data, e["m"], e["v"], e["last"], ids, self.t, self._cfg(e),
+                                    ignore_id=ignore_id, ignore_n=ids.numel() if ignore_id >= 0 else 0,
+                                    state_ld=e["state_ld"])
 
     def flush(self) -> None:
-        """bring every row of every exact table up to the current step (before evaluation, saving, reading weights)"""
-        if not self.exact_dense:
+        """bring every row of every exact table up to the current step (before evaluation, saving, reading weights);
+        a no-op when no step was taken since the last flush"""
+        if not self.exact_dense or self._flushed_at == self.t:
             return
         for e in self._entries:
-            if "last" in e and self.t > 0:
-                self._advance(e, None, self.t)
+            if "last" in e:
+                ops.adam_exact_advance(e["p"].data, e["m"], e["v"], e["last"], self.t, self._cfg(e),
+                                       state_ld=e["state_ld"])
+        self._flushed_at = self.t
 
     # -- torch.optim-like surface used by BaseRunner.fit ------------------------------------------------
     def zero_grad(self, set_to_none: bool = True) -> None:
@@ -145,12 +157,12 @@ class RowSparseOptimizer:
                 ids = pend[0][0] if len(pend) == 1 else torch.cat([pend[0][0], pend[1][0]])
                 ign = pend[0][2]
                 if "last" in e:
-                    # exact dense-Adam mode: the rows about to be updated must stand at step t-1 (they do already if
-                    # before_forward ran) and are stamped t, the step the update below applies
-                    upd = torch.unique(ids)
-                    if ign >= 0:
-                        upd = upd[upd != ign]            # padding positions are dropped by the plan: that row is not updated
-                    self._advance(e, upd, self.t - 1, stamp=self.t)
+                    # exact dense-Adam mode: the rows about to be updated must stand at step t-1 (they do already:
+                    # the forward that parked these streams caught them up) and are stamped t, the step the update
+                    # below applies; the plan's padding rule (ignore id in the first stream only) is the catch-up's
+                    ops.adam_exact_catch_up(p.data, e["m"], e["v"], e["last"], ids, self.t - 1, self._cfg(e),
+                                            stamp=self.t, ignore_id=ign, ignore_n=pend[0][0].numel() if ign >= 0 else 0,
+                                            state_ld=e["state_ld"])
                 plan = ops.make_plan(ids, p.shape[0], p.shape[1], ign, pend[0][0].numel() if ign >= 0 else 0)
                 plan.apply_optimizer(p.data, e["m"], e["v"], self._opt(e["wd"], e["state_ld"]), [x[1] for x in pend])
                 pend.clear()
@@ -182,6 +194,7 @@ class RowSparseOptimizer:
 
     def load_state_dict(self, sd: Dict) -> None:
         self.t = int(sd["t"])
+        self._flushed_at = -1
         for e in self._entries:
             st = sd["state"].get(e["name"])
             if st is None:

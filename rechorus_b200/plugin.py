@@ -162,6 +162,20 @@ class _KernelModelMixin:
         if getattr(opt, "exact_dense", False) and not self.training:
             opt.flush()                     # exact dense-Adam mode: ranks and lists must see rows advanced through skipped steps
 
+    def _exact_catch_up(self, *reads) -> None:
+        """Exact dense-Adam mode (RowSparseOptimizer(exact_dense=True)): a training forward first advances the rows it is
+        about to read -- each of ``reads`` is (table, ids) or (table, ids, ignore id) -- through the optimizer steps they
+        skipped, on the device and without a host synchronisation; an eval-mode forward (the host predict route through
+        ``inference``) flushes every table instead.  A no-op in the lazy mode."""
+        opt = self.__dict__.get("_b2r_optimizer")
+        if not getattr(opt, "exact_dense", False):
+            return
+        if self.training:
+            for r in reads:
+                opt.before_forward(*r)
+        else:
+            opt.flush()
+
     def has_query_rows(self) -> bool:
         """whether this model scores candidates as dot products with item-table rows (query_rows is overridden)"""
         return type(self).query_rows is not _KernelModelMixin.query_rows
@@ -219,13 +233,7 @@ class BPRMFKernels(_KernelModelMixin):
         self.check_list = []
         u_ids = feed_dict["user_id"]        # [B]
         i_ids = feed_dict["item_id"]        # [B, C]
-        opt = self.__dict__.get("_b2r_optimizer")
-        if getattr(opt, "exact_dense", False):                        # exact dense-Adam mode (next-round groundwork)
-            if self.training:
-                opt.before_forward(self.u_embeddings.weight, u_ids)
-                opt.before_forward(self.i_embeddings.weight, i_ids)
-            else:
-                opt.flush()
+        self._exact_catch_up((self.u_embeddings.weight, u_ids), (self.i_embeddings.weight, i_ids))
         u = ops.embedding(self.u_embeddings.weight, u_ids)            # [B, d]   (gather kernel)
         pred = ops.score(u, self.i_embeddings.weight, i_ids)          # [B, C]   (gather + dot kernel)
         out = {"prediction": pred.view(feed_dict["batch_size"], -1)}
@@ -246,10 +254,10 @@ class BPRMFKernels(_KernelModelMixin):
         Needs ``self.optimizer`` to be a ``RowSparseOptimizer``.  ``next_feed_dict`` (optional) is the next
         batch, already on the device: its index plan is prefetched while this step runs.  Returns the loss as a
         device scalar."""
-        if (self.emb_size not in (32, 64, 128) or getattr(self.optimizer, "exact_dense", False)
+        if (self.emb_size not in (32, 64, 128)
                 or not ops.DirectPlan.available(feed_dict["item_id"].numel(), self.item_num)):
-            # no plan/apply kernel for this width, the exact dense-Adam mode (which the single-call step does not
-            # implement yet), or a batch too large for the step's index plans: same step through the autograd nodes
+            # no plan/apply kernel for this width, or a batch too large for the step's index plans: same step through
+            # the autograd nodes
             self.optimizer.zero_grad()
             loss = self.loss(self.forward(feed_dict))
             loss.backward()
@@ -309,6 +317,8 @@ class NeuMFKernels(_KernelModelMixin):
         i_ids = feed_dict["item_id"]        # [B, C]
         B, C = i_ids.shape
         d = self.emb_size
+        self._exact_catch_up((self.mf_u_embeddings.weight, u_ids), (self.mf_i_embeddings.weight, i_ids),
+                             (self.mlp_u_embeddings.weight, u_ids), (self.mlp_i_embeddings.weight, i_ids))
         w_out = self.prediction.weight      # [1, d + last]: GMF part first, MLP part second (NeuMF.py:74)
         # GMF branch: sum_k w[k] * mf_u[b,k] * mf_i[id,k]  == rowdot(w * mf_u[b], mf_i[id])
         mf_u = ops.embedding(self.mf_u_embeddings.weight, u_ids)
@@ -508,6 +518,8 @@ class SASRecKernels(_KernelModelMixin):
         i_ids = feed_dict["item_id"]            # [B, C]
         history = feed_dict["history_items"]    # [B, Lb] right-padded with 0
         lengths = feed_dict["lengths"]          # [B]
+        # history padding (id 0) is never updated by the plan and feeds dead positions only: the flush catches row 0 up
+        self._exact_catch_up((self.i_embeddings.weight, history, 0), (self.i_embeddings.weight, i_ids))
         h = self.user_state(history, lengths, self._dropout_snapshot(history.device))
         pred = ops.score(h, self.i_embeddings.weight, i_ids)
         out = {"prediction": pred.view(history.shape[0], -1)}
@@ -595,6 +607,9 @@ class BaseModel(nn.Module):
         return [{"params": weight_p}, {"params": bias_p, "weight_decay": 0}]
 
     def save_model(self, model_path=None):
+        opt = self.__dict__.get("_b2r_optimizer")
+        if getattr(opt, "exact_dense", False):
+            opt.flush()                     # the checkpoint holds dense-Adam weights in either train or eval mode
         model_path = model_path or self.model_path
         d = os.path.dirname(model_path)
         if d:
