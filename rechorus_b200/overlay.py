@@ -28,7 +28,8 @@ def _make_runner_module(ref_runner_cls):
     untouched) with two seams re-pointed at the kernels, selected by flags the unchanged ``main.py`` parses for us
     (``main.py:164-176`` resolves the runner by the model's ``runner`` attribute and lets it add arguments):
       --fused_step 1      fit() = one C call per batch (model.train_step: forward, loss, backward, row-sparse optimizer;
-                          next batch's index plan prefetched) instead of the loop body of BaseRunner.py:185-207;
+                          next batch's index plan prefetched) instead of the loop body of BaseRunner.py:185-207
+                          (fit() takes the stand-alone runner's dispatch, runner._routed_fit);
       --device_metrics 1  evaluate() ranks on the GPU (model.eval_ranks) instead of shipping predictions to the host;
       --device_batches N  fit() = the epoch's negatives, row shuffle and collate (SASRec's histories included) as device
                           kernels, seed N (runner.BaseRunner.fit_on_device) on the reference's own Dataset and corpus;
@@ -38,7 +39,6 @@ def _make_runner_module(ref_runner_cls):
     import types
 
     from . import runner as ours
-    from .optim import RowSparseOptimizer
 
     class B200Runner(ref_runner_cls):
         @staticmethod
@@ -66,15 +66,8 @@ def _make_runner_module(ref_runner_cls):
                 _install_device_rec()
 
         def fit(self, dataset, epoch=-1):
-            model = dataset.model
-            if self.device_batches:
-                return ours.BaseRunner.fit_on_device(self, dataset, epoch)
-            if (self.fused_step and hasattr(model, "train_step")
-                    and isinstance(model.optimizer, RowSparseOptimizer)):       # the lazily-built fused optimizer
-                dataset.actions_before_epoch()                                  # BaseRunner.py:178: negatives
-                model.train()
-                return ours.BaseRunner._fit_whole_steps(self, dataset, epoch)
-            return super().fit(dataset, epoch)
+            loss = ours._routed_fit(self, dataset, epoch)
+            return super().fit(dataset, epoch) if loss is None else loss
 
         def evaluate(self, dataset, topks, metrics):
             if self.device_metrics and hasattr(dataset.model, "eval_ranks"):

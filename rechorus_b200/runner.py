@@ -2,7 +2,9 @@
 reference checkout: same flags, same ``train / fit / evaluate / predict / evaluate_method / print_res``
 semantics, same CPU RNG stream for the per-batch candidate shuffle.  Additions (all opt-in flags):
 ``--fused_optimizer 1`` installs ``RowSparseOptimizer`` through the ``model.optimizer`` seam
-(BaseRunner.py:176-177) and switches the embedding tables to 'fused' gradient mode.
+(BaseRunner.py:176-177) and switches the embedding tables to 'fused' gradient mode.  Every kernel route of a training
+epoch is one step loop, ``train_steps``, fed by ``host_batches`` (the reference's DataLoader) or ``device_batches``;
+``fit`` and ``fit_on_device`` pick the source and the step, and ``fit`` keeps the reference's loop for everything else.
 """
 from __future__ import annotations
 
@@ -18,6 +20,7 @@ import torch
 from torch.utils.data import DataLoader
 
 from . import ops
+from .graph import GraphedStep
 from .optim import RowSparseOptimizer
 
 
@@ -435,6 +438,173 @@ def write_rec_csv(runner, dataset, result_path: str, topk: int, sep: str, style:
         raise
 
 
+def train_steps(model, feeds, mode: str, batch_size: int, fill=None) -> List[torch.Tensor]:
+    """One training epoch over ``feeds`` (device feed dicts in epoch order, from ``host_batches`` or ``device_batches``):
+    the step loop of every kernel route.  Returns the steps' losses as device scalars.  ``mode`` is the loop body
+    (helpers/BaseRunner.py:193-206): "step", the model's one-call ``train_step``, given the next batch when it has the
+    same shape so that its index plan is built during this step; "graph", the step captured in a CUDA graph (GraphedStep,
+    cached in the model) on the first batch of ``batch_size`` rows, whose warm-up step trains that batch, and replayed for
+    every batch of the captured shape, while other shapes (the ragged last batch, a host SASRec batch of another width)
+    step eagerly; or "eager", zero_grad / forward / loss / backward / optimizer.step.  The next batch is taken before the
+    current step is enqueued; prefetched step plans are dropped before and after the epoch, and ids polled at its end.
+
+    ``fill`` (graph mode on device batches): full batches come unwritten and ``fill(dst, i)`` collates batch i into dst
+    just before its step, straight into the captured inputs for a replay.  They all share one shape, so a cached graph
+    that does not match them is captured again; without ``fill`` such a batch steps eagerly."""
+    losses = []
+    it = iter(feeds)
+    cur = next(it, None)
+    ops.bprmf_step_reset()
+    try:
+        i = 0
+        while cur is not None:
+            nxt = next(it, None)
+            gs = model.__dict__.get("_b2r_graphed_step") if mode == "graph" else None
+            full = mode == "graph" and cur["item_id"].shape[0] == batch_size
+            if mode == "step":
+                same = nxt is not None and nxt["item_id"].shape == cur["item_id"].shape
+                loss = model.train_step(cur, nxt if same else None)
+            elif full and (gs is None or (fill is not None and not gs.matches(cur))):
+                if fill is not None:
+                    fill(cur, i)
+                gs = model.__dict__["_b2r_graphed_step"] = GraphedStep(model, cur, warmup=1)
+                loss = gs.warmup_losses[0]                            # its warm-up step IS this batch's training step
+            elif gs is not None and gs.matches(cur):
+                if fill is not None:
+                    fill(gs.static, i)       # on the current stream: after the previous replay has read the inputs
+                    loss = gs.replay().clone()
+                else:
+                    loss = gs(cur).clone()
+            else:
+                model.optimizer.zero_grad()
+                loss = model.loss(model(cur))
+                loss.backward()
+                model.optimizer.step()
+                loss = loss.detach()
+            losses.append(loss)
+            cur = nxt
+            i += 1
+        if mode == "graph":
+            model.optimizer.sync_clock()
+    finally:
+        ops.bprmf_step_reset()
+    _poll_ids(model)
+    return losses
+
+
+def host_batches(runner, dataset):
+    """The batches of one epoch as the reference's fit builds them (helpers/BaseRunner.py:181-190): its DataLoader, each
+    batch moved to the device.  The per-row candidate permutation of :189 is drawn from the CPU generator, so the torch
+    RNG stream stays in step with the reference loop, but not applied: that is a no-op for candidates scored
+    independently, and the whole-step kernel wants the positive in column 0.  With dropout it is still one in
+    distribution: every element's mask is drawn independently (keyed by its position, not by the candidate's identity),
+    so permuting the candidate columns leaves the distribution of the step unchanged."""
+    dl = DataLoader(dataset, batch_size=runner.batch_size, shuffle=True, num_workers=runner.num_workers,
+                    collate_fn=dataset.collate_batch, pin_memory=bool(runner.pin_memory))
+    for batch in dl:
+        batch = batch_to_device(batch, dataset.model.device)
+        torch.rand(*batch["item_id"].shape)
+        yield batch
+
+
+def _collate_train(dataset, dst, start: int, Bn: int) -> None:
+    # rows [start, start + Bn) of device_batches' current epoch into the buffers dst: user / candidate columns, history
+    st = dataset.__dict__["_b2r_dev"]
+    ops.collate_general(st["users"], st["items"], st["neg"], st["perm"], start, Bn, dst["user_id"], dst["item_id"])
+    if "history" in st:
+        st["history"].collate(st["users"], st["perm"], start, Bn, dst["history_items"], dst["lengths"])
+
+
+def device_batches(runner, dataset, defer_full=False):
+    """SURVEY.md §8 row f3: the batches of one epoch built on the GPU (``--device_batches <seed>``), in epoch order.  What
+    the reference does on the host -- draw the negatives (models/BaseModel.py:206-214), shuffle the rows (the
+    DataLoader's RandomSampler), build one feed dict per sample and collate them (BaseModel.py:192-203,135-152) --
+    becomes three device operations: ``b2r_sample_negatives`` (one Philox draw + one binary search per negative, the
+    reference's distribution from a counter-based stream), a device permutation, and ``b2r_collate_general`` per batch.
+
+    Sequential datasets (models with ``history_max``, e.g. SASRec) also get ``history_items [B, Lp]`` and ``lengths [B]``
+    from ``b2r_collate_history`` (the slice of BaseModel.py:236-245 out of a device CSR of ``corpus.user_his``,
+    ops.DeviceHistory).  Every batch is right-padded to the fixed width Lp = min(history_max, max position), not to the
+    batch maximum as collate_batch does: the extra padding is dead work for SASRec (exact), and every full batch has the
+    same shape.  ``history_times`` is not produced; no kernel-backed model reads it.
+
+    The batches rotate through three buffers (current, next, one being refilled): a batch's step must be enqueued on the
+    current stream before the batch three places later is requested.  With ``defer_full`` the full batches are yielded
+    unwritten, for a consumer that collates each itself with ``_collate_train`` (train_steps' graph mode).
+
+    RNG: the host streams of the reference are NOT reproduced (a sequential NumPy / torch CPU stream cannot be drawn in
+    parallel); the epoch's negatives and order are reproducible from (seed, epoch)."""
+    model = dataset.model
+    dev = model.device
+    st = dataset.__dict__.get("_b2r_dev")
+    if st is None:
+        corpus = dataset.corpus
+        seed = int(runner.device_batches) if int(runner.device_batches) > 1 else 2023
+        st = {"users": torch.as_tensor(np.asarray(dataset.data["user_id"], dtype=np.int64)).to(dev),
+              "items": torch.as_tensor(np.asarray(dataset.data["item_id"], dtype=np.int64)).to(dev),
+              "sampler": ops.DeviceNegativeSampler(corpus.train_clicked_set, corpus.n_users, corpus.n_items, dev, seed=seed),
+              "gen": torch.Generator(device=dev), "seed": seed, "epoch": 0}
+        if hasattr(model, "history_max"):
+            st["history"] = ops.DeviceHistory(corpus.user_his, corpus.n_users, dataset.data["user_id"],
+                                              dataset.data["position"], model.history_max, dev)
+        dataset.__dict__["_b2r_dev"] = st
+    st["epoch"] += 1
+    N, K, B = st["users"].numel(), int(model.num_neg), int(runner.batch_size)
+    st["neg"] = st["perm"] = None                                              # the last epoch's, freed before these are drawn
+    st["neg"] = st["sampler"].sample(st["users"], K, st["epoch"])              # [N, K] int64 on the device
+    st["gen"].manual_seed(st["seed"] * 1_000_003 + st["epoch"])
+    st["perm"] = torch.randperm(N, device=dev, generator=st["gen"])
+    his = st.get("history")
+
+    def new_buf():
+        buf = {"user_id": torch.empty(B, dtype=torch.int64, device=dev),
+               "item_id": torch.empty((B, K + 1), dtype=torch.int64, device=dev), "batch_size": B, "phase": "train"}
+        if his is not None:
+            buf["history_items"] = torch.empty((B, his.width), dtype=torch.int64, device=dev)
+            buf["lengths"] = torch.empty(B, dtype=torch.int64, device=dev)
+        return buf
+
+    bufs = st.get("bufs")
+    if bufs is None or bufs[0]["item_id"].shape != (B, K + 1):
+        bufs = st["bufs"] = [new_buf() for _ in range(3)]
+    for k in range((N + B - 1) // B):
+        Bn = min(B, N - k * B)
+        buf = bufs[k % 3]
+        if Bn == B:
+            if not defer_full:
+                _collate_train(dataset, buf, k * B, B)
+            yield buf
+        else:
+            _collate_train(dataset, buf, k * B, Bn)
+            yield dict({key: (v[:Bn] if isinstance(v, torch.Tensor) else v) for key, v in buf.items()}, batch_size=Bn)
+
+
+def _routed_fit(runner, dataset, epoch=-1):
+    """The dispatch of BaseRunner.fit and of the overlay's B200Runner.fit (a subclass of the reference's BaseRunner that
+    lacks some of these flags, hence getattr): builds the optimizer and the --device_sampler, then returns the epoch's loss
+    when a flag routes it through train_steps -- fit_on_device, or host_batches with np.mean of the float32 losses, the
+    reference's reduction -- and None when the caller's own loop should run it."""
+    model = dataset.model
+    opt = model.optimizer
+    graph = getattr(runner, "graph_step", 0)
+    if opt is None or (graph and isinstance(opt, RowSparseOptimizer) and not opt._want_clock and opt.t == 0):
+        model.optimizer = runner._build_optimizer(model)     # (a lazily built one without the device clock is replaced)
+    seed = getattr(runner, "device_sampler", 0)
+    if seed and model.__dict__.get("_b2r_device_sampler") is None:
+        corpus = dataset.corpus
+        model.__dict__["_b2r_device_sampler"] = ops.DeviceNegativeSampler(
+            corpus.train_clicked_set, corpus.n_users, corpus.n_items, model.device, seed=seed)
+    if getattr(runner, "device_batches", 0):
+        return BaseRunner.fit_on_device(runner, dataset, epoch)
+    step = getattr(runner, "fused_step", 0) and hasattr(model, "train_step")
+    if not (step or graph) or not isinstance(model.optimizer, RowSparseOptimizer):
+        return None
+    dataset.actions_before_epoch()                                 # BaseRunner.py:178: the epoch's negatives
+    model.train()
+    losses = train_steps(model, host_batches(runner, dataset), "step" if step else "graph", runner.batch_size)
+    return float(np.mean(torch.stack([l.reshape(()) for l in losses]).cpu().numpy())) if losses else float("nan")
+
+
 class BaseRunner:
     @staticmethod
     def parse_runner_args(parser):
@@ -581,208 +751,32 @@ class BaseRunner:
             best + 1, format_metric(dev_results[best]), self.time[1] - self.time[0]))
         model.load_model()
 
-    def _fit_whole_steps(self, dataset, epoch=-1) -> float:
-        """The same epoch with the loop body of helpers/BaseRunner.py:185-207 replaced by the model's single-call
-        ``train_step`` (forward + loss + backward + row-sparse optimizer in one C call, the next batch's index plan
-        prefetched).  Batches and RNG consumption are those of ``fit``: the per-row candidate permutation is still
-        drawn (so the torch RNG stream stays in step with the reference loop) but not applied -- it is a no-op for a
-        model whose candidates are scored independently, and the whole-step kernel wants the positive in column 0.
-        Losses stay on the device until the epoch ends (the reference syncs on every step)."""
-        model = dataset.model
-        dl = DataLoader(dataset, batch_size=self.batch_size, shuffle=True, num_workers=self.num_workers,
-                        collate_fn=dataset.collate_batch, pin_memory=bool(self.pin_memory))
-        it = iter(dl)
-        cur = next(it, None)
-        cur = batch_to_device(cur, model.device) if cur is not None else None
-        losses = []
-        ops.bprmf_step_reset()                 # no plan prefetched by an earlier (possibly aborted) epoch survives
-        try:
-            while cur is not None:
-                nxt = next(it, None)
-                if nxt is not None:
-                    nxt = batch_to_device(nxt, model.device)
-                torch.rand(*cur["item_id"].shape)                     # BaseRunner.py:189's draw, see above
-                same_shape = nxt is not None and nxt["item_id"].shape == cur["item_id"].shape
-                losses.append(model.train_step(cur, nxt if same_shape else None))
-                cur = nxt
-        finally:
-            ops.bprmf_step_reset()
-        out = float(np.mean(torch.stack(losses).cpu().numpy())) if losses else float("nan")
-        _poll_ids(model)
-        return out
-
-    def _fit_graphed(self, dataset, epoch=-1) -> float:
-        """The same epoch with the loop body of helpers/BaseRunner.py:193-206 captured once in a CUDA graph
-        (rechorus_b200.graph.GraphedStep) and replayed for every batch of the captured shape: one launch per step instead of
-        ~70 (NeuMF) to ~150 (SASRec).  The first full-size batch trains through the capture's eager warm-up step; the ragged
-        last batch runs eagerly.  As in ``_fit_whole_steps`` the per-row candidate permutation of :189 is drawn (RNG stream in
-        step with the reference) but not applied: it is a no-op for candidates scored independently.  With dropout it is
-        still one in distribution: every element's mask is drawn independently (keyed by its position, not by the
-        candidate's identity), so permuting the candidate columns leaves the distribution of the step unchanged.  The
-        dropout step counter lives on the device and advances on every replay."""
-        from .graph import GraphedStep
-        model = dataset.model
-        dl = DataLoader(dataset, batch_size=self.batch_size, shuffle=True, num_workers=self.num_workers,
-                        collate_fn=dataset.collate_batch, pin_memory=bool(self.pin_memory))
-        losses = []
-        for batch in dl:
-            batch = batch_to_device(batch, model.device)
-            torch.rand(*batch["item_id"].shape)                       # BaseRunner.py:189's draw
-            gs = model.__dict__.get("_b2r_graphed_step")
-            if gs is None and batch["item_id"].shape[0] == self.batch_size:
-                gs = GraphedStep(model, batch, warmup=1)              # its warm-up step IS this batch's training step
-                model.__dict__["_b2r_graphed_step"] = gs
-                losses.append(gs.warmup_losses[0])
-            elif gs is not None and gs.matches(batch):
-                losses.append(gs(batch).clone())
-            else:
-                model.optimizer.zero_grad()
-                loss = model.loss(model(batch))
-                loss.backward()
-                model.optimizer.step()
-                losses.append(loss.detach())
-        model.optimizer.sync_clock()                                  # the host step counter follows the device clock
-        out = float(np.mean(torch.stack([l.reshape(()) for l in losses]).cpu().numpy())) if losses else float("nan")
-        _poll_ids(model)
-        return out
-
     def fit_on_device(self, dataset, epoch=-1) -> float:
-        """SURVEY.md §8 row f3: the same epoch with BATCH PRODUCTION on the GPU (``--device_batches <seed>``).  What the
-        reference does on the host -- draw the negatives (models/BaseModel.py:206-214), shuffle the rows (the
-        DataLoader's RandomSampler), build one feed dict per sample and collate them (BaseModel.py:192-203,135-152) --
-        becomes three device operations: ``b2r_sample_negatives`` (one Philox draw + one binary search per negative, the
-        reference's distribution from a counter-based stream), a device permutation, and ``b2r_collate_general`` per
-        batch.  The training step is the model's ``train_step`` (one C call) or, for models without one, the plugin
-        contract's forward / loss / backward / optimizer.step on the device batch.
-
-        Sequential datasets (models with ``history_max``, e.g. SASRec) also get ``history_items [B, Lp]`` and ``lengths
-        [B]`` from ``b2r_collate_history`` (the slice of BaseModel.py:236-245 out of a device CSR of ``corpus.user_his``,
-        ops.DeviceHistory).  Every batch is right-padded to the fixed width Lp = min(history_max, max position), not to
-        the batch maximum as collate_batch does: the extra padding is dead work for SASRec (exact), and every full batch
-        has the same shape.  ``history_times`` is not produced; no kernel-backed model reads it.
-
-        ``--graph_step 1`` with a model without ``train_step`` (NeuMF, SASRec): the full-size batches are replayed through
-        one captured step (rechorus_b200.graph.GraphedStep), each collated straight into the captured inputs just before
-        its replay; the first full batch trains through the capture's warm-up step, the ragged last batch eagerly.
-
-        RNG: the host streams of the reference are NOT reproduced (a sequential NumPy / torch CPU stream cannot be drawn
-        in parallel); results are reproducible from (seed, epoch)."""
+        """The same epoch with batch production on the GPU (``--device_batches <seed>``): ``device_batches`` through
+        ``train_steps``, with the model's ``train_step`` when it has one, else with ``--graph_step 1`` the captured step
+        (full batches collated straight into its inputs), else eagerly.  Returns the mean of the steps' losses, taken on
+        the device."""
         model = dataset.model
         if model.optimizer is None:
             model.optimizer = self._build_optimizer(model)
-        dev = model.device
-        st = dataset.__dict__.get("_b2r_dev")
-        if st is None:
-            corpus = dataset.corpus
-            seed = int(self.device_batches) if int(self.device_batches) > 1 else 2023
-            st = {"users": torch.as_tensor(np.asarray(dataset.data["user_id"], dtype=np.int64)).to(dev),
-                  "items": torch.as_tensor(np.asarray(dataset.data["item_id"], dtype=np.int64)).to(dev),
-                  "sampler": ops.DeviceNegativeSampler(corpus.train_clicked_set, corpus.n_users, corpus.n_items, dev, seed=seed),
-                  "gen": torch.Generator(device=dev), "seed": seed, "epoch": 0}
-            if hasattr(model, "history_max"):
-                st["history"] = ops.DeviceHistory(corpus.user_his, corpus.n_users, dataset.data["user_id"],
-                                                  dataset.data["position"], model.history_max, dev)
-            dataset.__dict__["_b2r_dev"] = st
-        st["epoch"] += 1
-        N, K, B = st["users"].numel(), int(model.num_neg), int(self.batch_size)
-        neg = st["sampler"].sample(st["users"], K, st["epoch"])                     # [N, K] int64 on the device
-        st["gen"].manual_seed(st["seed"] * 1_000_003 + st["epoch"])
-        perm = torch.randperm(N, device=dev, generator=st["gen"])
         model.train()
-        use_step = hasattr(model, "train_step") and isinstance(model.optimizer, RowSparseOptimizer)
-        use_graph = (not use_step and bool(getattr(self, "graph_step", 0))
-                     and isinstance(model.optimizer, RowSparseOptimizer))
-        his = st.get("history")
-        n_steps = (N + B - 1) // B
-        NB = 3                                                                       # batch buffers: current, next, one being refilled
-
-        def new_buf():
-            buf = {"user_id": torch.empty(B, dtype=torch.int64, device=dev),
-                   "item_id": torch.empty((B, K + 1), dtype=torch.int64, device=dev), "batch_size": B, "phase": "train"}
-            if his is not None:
-                buf["history_items"] = torch.empty((B, his.width), dtype=torch.int64, device=dev)
-                buf["lengths"] = torch.empty(B, dtype=torch.int64, device=dev)
-            return buf
-
-        bufs = st.get("bufs")
-        if bufs is None or bufs[0]["item_id"].shape != (B, K + 1):
-            bufs = st["bufs"] = [new_buf() for _ in range(NB)]
-
-        def fill(buf, k, Bn):
-            # two launches: user / candidate columns, then (sequential models) the history
-            ops.collate_general(st["users"], st["items"], neg, perm, k * B, Bn, buf["user_id"], buf["item_id"])
-            if his is not None:
-                his.collate(st["users"], perm, k * B, Bn, buf["history_items"], buf["lengths"])
-
-        def batch(k):
-            Bn = min(B, N - k * B)
-            buf = bufs[k % NB]
-            fill(buf, k, Bn)
-            if Bn == B:
-                return buf
-            out = {key: (v[:Bn] if isinstance(v, torch.Tensor) else v) for key, v in buf.items()}
-            out["batch_size"] = Bn
-            return out
-
-        def eager_step(feed):
-            model.optimizer.zero_grad()
-            loss = model.loss(model(feed))
-            loss.backward()
-            model.optimizer.step()
-            return loss.detach()
-
-        losses = []
-        ops.bprmf_step_reset()
-        try:
-            if use_graph:
-                from .graph import GraphedStep
-                gs = model.__dict__.get("_b2r_graphed_step")
-                for k in range(n_steps):
-                    if N - k * B < B:
-                        losses.append(eager_step(batch(k)))                         # the ragged last batch
-                    elif gs is None or not gs.matches(bufs[0]):
-                        gs = GraphedStep(model, batch(k), warmup=1)                 # its warm-up step IS this batch's step
-                        model.__dict__["_b2r_graphed_step"] = gs
-                        losses.append(gs.warmup_losses[0])
-                    else:
-                        # straight into the captured inputs; on the same stream, so after the previous replay read them
-                        fill(gs.static, k, B)
-                        losses.append(gs.replay().clone())
-                model.optimizer.sync_clock()                                       # the host step counter follows the device clock
-            else:
-                cur = batch(0)
-                for k in range(n_steps):
-                    nxt = batch(k + 1) if k + 1 < n_steps else None
-                    if use_step:
-                        same = nxt is not None and nxt["item_id"].shape == cur["item_id"].shape
-                        losses.append(model.train_step(cur, nxt if same else None))
-                    else:
-                        losses.append(eager_step(cur))
-                    cur = nxt
-        finally:
-            ops.bprmf_step_reset()
-        out = float(torch.stack(losses).mean().cpu()) if losses else float("nan")
-        _poll_ids(model)
-        return out
+        fused = isinstance(model.optimizer, RowSparseOptimizer)
+        mode = "step" if fused and hasattr(model, "train_step") else \
+            "graph" if fused and getattr(self, "graph_step", 0) else "eager"
+        B = int(self.batch_size)
+        fill = (lambda dst, i: _collate_train(dataset, dst, i * B, B)) if mode == "graph" else None
+        losses = train_steps(model, device_batches(self, dataset, defer_full=fill is not None), mode, B, fill)
+        return float(torch.stack(losses).mean().cpu()) if losses else float("nan")
 
     def fit(self, dataset, epoch=-1) -> float:
-        """helpers/BaseRunner.py:174-208, step for step."""
+        """helpers/BaseRunner.py:174-208, step for step, unless a flag routes the epoch through ``train_steps``
+        (``_routed_fit``)."""
+        loss = _routed_fit(self, dataset, epoch)
+        if loss is not None:
+            return loss
         model = dataset.model
-        opt = model.optimizer
-        if opt is None or (self.graph_step and isinstance(opt, RowSparseOptimizer) and not opt._want_clock and opt.t == 0):
-            model.optimizer = self._build_optimizer(model)     # (a lazily built one without the device clock is replaced)
-        if self.device_sampler and model.__dict__.get("_b2r_device_sampler") is None:
-            corpus = dataset.corpus
-            model.__dict__["_b2r_device_sampler"] = ops.DeviceNegativeSampler(
-                corpus.train_clicked_set, corpus.n_users, corpus.n_items, model.device, seed=self.device_sampler)
-        if self.device_batches:
-            return self.fit_on_device(dataset, epoch)
         dataset.actions_before_epoch()
         model.train()
-        if self.fused_step and hasattr(model, "train_step") and isinstance(model.optimizer, RowSparseOptimizer):
-            return self._fit_whole_steps(dataset, epoch)
-        if self.graph_step and isinstance(model.optimizer, RowSparseOptimizer):
-            return self._fit_graphed(dataset, epoch)
         losses = []
         dl = DataLoader(dataset, batch_size=self.batch_size, shuffle=True, num_workers=self.num_workers,
                         collate_fn=dataset.collate_batch, pin_memory=bool(self.pin_memory))
